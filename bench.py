@@ -11,6 +11,10 @@ tests/golden/make_rpng_sim_cases.py from the host simulator with seeds 0). Other
 
 Prints ONE JSON line (rank 0). `value` = updates/s with inputs resident in HBM (CUDA events on the engine's stream, L2
 flushed between steps); `e2e` = updates/s through the C-ABI call with host buffers (H2D/D2H inside the timed call).
+
+--dump-outputs DIR writes what the last timed step returned to its caller (updated covariance, state correction, per-feature
+results) as DIR/<name>.npy in float64, all finite: points and chi2 only for the features that have them, with the features'
+indices in <name>_index.npy. The inputs are fixed by the config and seed 0, so two builds can be compared file by file.
 """
 from __future__ import annotations
 
@@ -28,20 +32,25 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-FP64_PEAK_TFLOPS = 37.1  # measured on this pool's B200s: DMMA m8n8k4 and DFMA both saturate at 64 FMA/clk/SM (tools/ubench/fp64_rate.cu,
-#                          profiles/ubench_r02.txt); MEASURED_PEAKS.json carries no FP64 entry
+FP64_PEAK_TFLOPS = 67.0  # H100 SXM data sheet: FP64 tensor core (DMMA), dense, at 700 W; not a measured rate
+FP64_PEAK_SOURCE = "H100 SXM data sheet, FP64 tensor core, dense, 700 W (power-limited cards clock lower)"
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
+
+
+def dump_outputs(d: str, arrays: dict):
+    bad = [name for name, a in arrays.items() if not np.isfinite(a).all()]
+    if bad:
+        raise SystemExit(f"bench.py: non-finite values in the outputs {bad}")
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks, power limit and throttle reasons during the timed region."""
 
     def __init__(self, index=0):
         self.index = index
@@ -52,7 +61,7 @@ class ClockSampler:
         try:
             self.path = tempfile.NamedTemporaryFile(delete=False, suffix=".csv").name
             q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
-                 "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+                 "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-lms", "50", "-i", str(self.index)],
                                          stdout=open(self.path, "w"), stderr=subprocess.DEVNULL)
         except Exception:
@@ -68,14 +77,15 @@ class ClockSampler:
             self.proc.wait(timeout=5)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        sm, mx, pl, reasons = [], [], [], set()
         try:
             for line in open(self.path):
                 f = [x.strip() for x in line.split(",")]
-                if len(f) < 9:
+                if len(f) < 10:
                     continue
                 sm.append(float(f[1]))
                 mx.append(float(f[2]))
+                pl.append(f[9])  # watts, or "[N/A]" where the driver does not report it
                 for name, v in zip(["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"], f[5:9]):
                     if v.lower().startswith("active"):
                         reasons.add(name)
@@ -83,7 +93,8 @@ class ClockSampler:
         except Exception:
             pass
         if sm:
-            out = {"sm_mhz": float(np.median(sm)), "sm_max_mhz": float(max(mx)), "reasons": sorted(reasons), "samples": len(sm)}
+            out = {"sm_mhz": float(np.median(sm)), "sm_max_mhz": float(max(mx)), "power_limit_w": pl[-1], "reasons": sorted(reasons),
+                   "samples": len(sm)}
         return out
 
 
@@ -205,13 +216,9 @@ def run_reference(args, rank):
         print(json.dumps({"impl": "reference", "unavailable": "config 5 is a kernel microbenchmark; the reference arm runs the update configs"}))
         return
     budget_steps = args.steps
-    # bounded sample: at most ~150 s of CPU work
-    t_probe = time.perf_counter()
-    ups0, r, _ = cpu_updates(w, 1, warm=0)
-    t_one = time.perf_counter() - t_probe
-    budget_steps = int(max(3, min(args.steps, 150.0 / max(t_one, 1e-3))))
-    old = pin_to_one_core()
     from oracle import ovo_py
+    ovo_py.build()
+    old = pin_to_one_core()
     try:
         for _ in range(min(args.warmup, 1)):
             ovo_py.msckf_update(w.frame, w.feats, w.opts, w.P, dumps=False)
@@ -252,6 +259,8 @@ def quiet_stdout():
 
 def emit(line: dict):
     global _SAVED_STDOUT
+    import torch
+    line["gpu"] = torch.cuda.get_device_name()  # absolute numbers belong to the card they were measured on
     sys.stdout.flush()
     if _SAVED_STDOUT is not None:
         os.dup2(_SAVED_STDOUT, 1)
@@ -291,17 +300,6 @@ def kernel_table(eng, w: Workload, repeats=5):
     return [{"kernel": s, "launches": acc[s][0][0], "us_per_step": float(np.median([t for _, t in acc[s]]))} for s in order]
 
 
-def ncu_traffic(kernel: str):
-    """dram bytes (read + write) per launch of `kernel` from the committed ncu --set full summary of this round, or None."""
-    p = os.path.join(ROOT, "profiles", "ncu_r02_summary.json")
-    try:
-        d = json.load(open(p))
-        k = d["kernels"][kernel]
-        return float(k["dram_bytes_read"] + k["dram_bytes_write"]), f"profiles/ncu_r02_summary.json ({d.get('how', 'ncu --set full, cold cache')})"
-    except Exception:
-        return None, None
-
-
 def rooflines(w: Workload, stats, stage_ms, ktab, nt_cols):
     """Roofline entries: the dominant kernel first (contract key `roofline`), then one entry per remaining heavy kernel."""
     hbm_peak, peak_src = peaks()
@@ -314,10 +312,9 @@ def rooflines(w: Workload, stats, stage_ms, ktab, nt_cols):
     if "k_feature_system" in kt:
         t = stage_ms[1] * 1e-3  # the size classes run concurrently on three streams: the stage time IS the kernel group's duration
         by = 8.0 * m_all * (nt_cols) + 20.0 * int(M.sum())
-        tr, src = ncu_traffic("k_feature_system")
         out.append({"kernel": "k_feature_system (Jacobians + nullspace projection + chi2 gate, one CTA per feature; 3 size-class launches side by side)",
-                    "bound": "hbm", "achieved": by / t / 1e9, "peak": hbm_peak, "unit": "GB/s", "frac": by / t / 1e9 / hbm_peak, "traffic": tr,
-                    "traffic_source": src, "peak_source": peak_src, "launches_per_step": kt["k_feature_system"]["launches"],
+                    "bound": "hbm", "achieved": by / t / 1e9, "peak": hbm_peak, "unit": "GB/s", "frac": by / t / 1e9 / hbm_peak, "traffic": None,
+                    "peak_source": peak_src, "launches_per_step": kt["k_feature_system"]["launches"],
                     "avg_launch_us": 1e6 * t, "algorithmic_bytes_per_launch": by,
                     "note": "algorithmic bytes = 8 B x staged rows x (n+1) written + 20 B/measurement read; the stage is bound by the latency of the longest "
                             "tracks' CTAs (chi2 Cholesky pivot chain, sparse S accumulation), not by HBM"})
@@ -325,10 +322,8 @@ def rooflines(w: Workload, stats, stage_ms, ktab, nt_cols):
         if kname not in kt:
             return
         t = kt[kname]["us_per_step"] * 1e-6
-        tr, src = ncu_traffic(kname)
         out.append({"kernel": label, "bound": "tensor", "achieved": flops / t / 1e12, "peak": FP64_PEAK_TFLOPS, "unit": "TFLOP/s",
-                    "frac": flops / t / 1e12 / FP64_PEAK_TFLOPS, "traffic": tr, "traffic_source": src,
-                    "peak_source": "FP64 DMMA/DFMA rate measured with tools/ubench/fp64_rate.cu on this pool (no FP64 entry in MEASURED_PEAKS.json)",
+                    "frac": flops / t / 1e12 / FP64_PEAK_TFLOPS, "traffic": None, "peak_source": FP64_PEAK_SOURCE,
                     "launches_per_step": kt[kname]["launches"], "avg_launch_us": 1e6 * t / kt[kname]["launches"], "flops_per_step": flops, "note": extra})
     nT = (nt_cols + 31) // 32
     fp64("k_cq_gram", "k_cq_gram (Gram matrix of the stacked system on the FP64 tensor pipe, DMMA m8n8k4; two passes)",
@@ -336,7 +331,7 @@ def rooflines(w: Workload, stats, stage_ms, ktab, nt_cols):
     fp64("k_cq_trsm", "k_cq_trsm (A <- A R^-1 in registers, DMMA pushes + per-row substitution; stacked system once, EKF gain once)",
          1.0 * (m_all + w.P.shape[0]) * nt_cols * nt_cols, "flops = rows x n^2 (triangular solve)")
     fp64("k_cq_chol_gram", "k_cq_chol_gram (single-CTA DMMA Cholesky, 155 x 155, two passes)", 2 * nt_cols**3 / 3.0,
-         "latency-bound by the 155-pivot chain (about 125 cycles per pivot), not by the pipe")
+         "latency-bound by the 155-pivot chain, not by the pipe")
     return out
 
 
@@ -379,6 +374,7 @@ def bench_update(args, w: Workload, local_rank=0, dist=None, rank=0, world=1):
     barrier()
     ms, stage_sum = eng.msckf_replay(W + K, flush_l2=True)
     barrier()
+    P_out = eng.cov_get()  # covariance after the last replayed update (outside the timed bracket)
     clocks = sampler.stop() if rank == 0 else None
     ms = ms[W:]
     t_dev = float(ms.sum()) * 1e-3
@@ -387,7 +383,8 @@ def bench_update(args, w: Workload, local_rank=0, dist=None, rank=0, world=1):
         tt = torch.tensor([t_e2e, t_dev], dtype=torch.float64, device=torch.device("cuda", local_rank))
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
         t_e2e, t_dev = float(tt[0]), float(tt[1])
-    return dict(eng=eng, K=K, W=W, t_e2e=t_e2e, t_dev=t_dev, stage_ms=stage_ms, stats=stats, out=out, cnt=cnt, clocks=clocks, ms=ms)
+    return dict(eng=eng, K=K, W=W, t_e2e=t_e2e, t_dev=t_dev, stage_ms=stage_ms, stats=stats, out=out, dx=dx, P=P_out, cnt=cnt, clocks=clocks,
+                ms=ms)
 
 
 def bench_dense(args, w: Workload, local_rank=0):
@@ -396,7 +393,7 @@ def bench_dense(args, w: Workload, local_rank=0):
     import torch
     from open_vins_b200 import capi
     eng = capi.Engine(max_state=512, max_feats=64, max_meas=4096, max_rows=8192, device=local_rank)
-    K, W = max(5, min(args.steps, 50)), args.warmup
+    K, W = args.steps, args.warmup
     n = w.H.shape[1]
     for _ in range(W):
         eng.cov_set(w.P)
@@ -405,8 +402,9 @@ def bench_dense(args, w: Workload, local_rank=0):
     t0 = time.perf_counter()
     for _ in range(K):
         eng.cov_set(w.P)
-        eng.ekf_update([0], [n], w.H, w.res, sigma2=1.0)
+        _, dx = eng.ekf_update([0], [n], w.H, w.res, sigma2=1.0)
     dt = (time.perf_counter() - t0) / K
+    outputs = {"P": eng.cov_get(), "dx": dx}
     eng.set_profile(True)
     sums, prof = [], None
     for _ in range(5):
@@ -416,7 +414,7 @@ def bench_dense(args, w: Workload, local_rank=0):
         sums.append(sum(us for _, us in prof))
     eng.set_profile(False)
     eng.close()
-    return dt, K, W, prof, float(np.median(sums)) * 1e-6
+    return dt, K, W, prof, float(np.median(sums)) * 1e-6, outputs
 
 
 def main():
@@ -431,6 +429,7 @@ def main():
                     help="measurement compression: cholqr2 (default, csrc/k_cholqr.cu), tsqr (Householder), gram (one-pass normal equations)")
     ap.add_argument("--features", type=int, default=None, help="synthetic batch with this many features instead of the config's captured case")
     ap.add_argument("--no-sweep", action="store_true", help="N>1: skip the 4096-feature sharded sweep point")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's results as DIR/<name>.npy (float64)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))
@@ -456,7 +455,9 @@ def main():
 
     if w.mode == "dense":
         if rank == 0:
-            dt, K, W, prof, t_kernels = bench_dense(args, w, local_rank)
+            dt, K, W, prof, t_kernels, outputs = bench_dense(args, w, local_rank)
+            if args.dump_outputs:
+                dump_outputs(args.dump_outputs, outputs)
             m, n = w.H.shape
             flops = 2.0 * m * n * n - (2.0 / 3.0) * n**3 + 4.0 * m * n + 2.0 * n * n * n + 2 * n**3 / 3.0 + 3.0 * n**3
             ktab = {}
@@ -538,7 +539,18 @@ def main():
                 "roofline": rl[0] if rl else None, "rooflines": rl[1:],
                 "clocks": r["clocks"],
             }
+            if args.dump_outputs:
+                o = r["out"]
+                arrays = {"P": r["P"], "dx": r["dx"], "feat_status": o.status, "feat_anchor_cam": o.anchor_cam, "feat_anchor_clone": o.anchor_clone}
+                # a feature dropped before triangulation or the gate has no point / chi2 (NaN in FeatOut): write the rows that were
+                # computed and, beside them, which features they belong to
+                for name, a in (("feat_p_FinG", o.p_FinG), ("feat_p_FinA", o.p_FinA), ("feat_chi2", o.chi2)):
+                    rows = np.isfinite(a.reshape(len(a), -1)).all(axis=1)
+                    arrays[name], arrays[name + "_index"] = a[rows], np.flatnonzero(rows)
+                dump_outputs(args.dump_outputs, arrays)
     else:
+        if args.dump_outputs:
+            raise SystemExit("bench.py: --dump-outputs covers the single-GPU and replicated update paths, not the sharded one")
         # sharded: features over ranks, ONE all-gather of the compressed blocks per update
         cap = max(1024, F)
         eng = capi.Engine(max_state=w.max_state, max_feats=cap, max_meas=cap * 64, device=local_rank)

@@ -1,8 +1,8 @@
 /*
- * ovb200.h — C ABI of the B200-native MSCKF update engine (libovb200.so).
+ * ovb200.h — C ABI of the H100-native MSCKF update engine (libovb200.so).
  *
  * This is the drop-in boundary for the ONE hot path of rpng/open_vins that this
- * repo re-implements for sm_100a:   UpdaterMSCKF::update  →  triangulate →
+ * repo re-implements for sm_90a:    UpdaterMSCKF::update  →  triangulate →
  * Jacobian → nullspace → chi² gate → stack → compress → EKFUpdate,  plus the
  * covariance side of Propagator::propagate_and_clone (EKFPropagation, clone,
  * marginalize).  The reference has no FFI layer; the seam is its C++ class

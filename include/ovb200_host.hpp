@@ -137,7 +137,7 @@ public:
   State(const StateOptions &options, const ovb_config &cfg) : _options(options) {
     ovb_status st = ovb_create(&cfg, &_ctx);
     if (st != OVB_OK)
-      throw Error(st, std::string("ovb_create: ") + (_ctx ? ovb_last_error(_ctx) : "no context (is a B200 visible?)"));
+      throw Error(st, std::string("ovb_create: ") + (_ctx ? ovb_last_error(_ctx) : "no context (is a CUDA GPU visible?)"));
     _cameras.resize((size_t)options.num_cameras);
   }
   ~State() {

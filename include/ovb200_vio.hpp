@@ -54,7 +54,7 @@ public:
   explicit EngineCov(const ovb_config &cfg) {
     const ovb_status st = ovb_create(&cfg, &ctx_);
     if (st != OVB_OK)
-      throw Error(st, std::string("ovb_create: ") + (ctx_ ? ovb_last_error(ctx_) : "no context (is a B200 visible?)"));
+      throw Error(st, std::string("ovb_create: ") + (ctx_ ? ovb_last_error(ctx_) : "no context (is a CUDA GPU visible?)"));
   }
   ~EngineCov() override {
     if (ctx_)

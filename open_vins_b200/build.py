@@ -1,4 +1,4 @@
-"""Build libovb200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libovb200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
 Per-feature geometry (k_triangulate.cu, k_feature.cu) is compiled with -fmad=false so its rounding sequence follows the
 reference's non-FMA Eigen arithmetic (SURVEY.md App. A.11); the dense algebra (TSQR, EKF) keeps FMA contraction.
@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libovb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 UNITS = [

@@ -235,7 +235,7 @@ def load_library(path: str | None = None) -> C.CDLL:
         return _LIB
     p = path or LIB_PATH
     if not os.path.exists(p):
-        raise RuntimeError(f"{p} not found — run `python -m open_vins_b200.build` (nvcc, sm_100a). "
+        raise RuntimeError(f"{p} not found — run `python -m open_vins_b200.build` (nvcc, sm_90a). "
                            "The engine has no CPU fallback.")
     lib = C.CDLL(p)
     vp = C.c_void_p

@@ -57,9 +57,9 @@ __device__ __forceinline__ CtView ct_view_carve(double *base, int NRB, int *flag
 // (semidefinite input) and a zero pivot empties its column. Rows >= nbk of the tile (right-hand-side rows sharing the last
 // diagonal tile) come out solved against the nbk x nbk factor; columns >= nbk come out zero. invd[0..8) <- 1/L_jj.
 //
-// What the eight pivots cost is their dependent chain; measured on B200 (tools/ubench/diag8_bench.cu): 2200 cycles when
-// every lane factors the whole block in registers (~450 FP64 instructions, in-order issue puts them on the chain), 1370
-// with the block spread over the lanes and column j broadcast after scaling, and the form below, where
+// What the eight pivots cost is their dependent chain (tools/ubench/diag8_bench.cu times it). It is longest when every
+// lane factors the whole block in registers (~450 FP64 instructions, in-order issue puts them on the chain), shorter with
+// the block spread over the lanes and column j broadcast after scaling, and shortest in the form below, where
 //   * the UNSCALED column j and the next diagonal entry are broadcast at the top of the step (the shuffles run under the
 //     reciprocal square root), each lane scaling what it receives (same inputs, same rounding: bit-identical), and
 //   * every lane carries the next pivot itself (p' = a[j+1][j+1] - (a[j+1][j] iv)^2, exactly what the owning lane computes),

@@ -4,7 +4,7 @@
 // (ov_msckf/src/state/StateHelper.cpp:226-254) and the chi² test + stacking of UpdaterMSCKF::update
 // (ov_msckf/src/update/UpdaterMSCKF.cpp:196-256).
 //
-// B200-first formulation (not the reference's dense Eigen path):
+// GPU-first formulation (not the reference's dense Eigen path):
 //  * the per-measurement Jacobian is kept block-sparse in shared memory (clone 2x6 | extrinsics 2x6 | intrinsics 2x8
 //    [| anchor clone 2x6 | anchor extrinsics 2x6]) — 600 B per measurement instead of 2 x w_f doubles;
 //  * the left nullspace of H_f is applied as a rank-3 compact-WY reflector (three Householder vectors) instead of

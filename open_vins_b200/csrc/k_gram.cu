@@ -10,7 +10,7 @@
 // is rank deficient (global position/yaw gauge, SURVEY.md App. A.6): pivots at round-off level are zeroed (semidefinite
 // Cholesky) instead of failing; the reference's Givens sweep leaves O(eps |H|) noise rows in their place.
 //
-// Why it is the B200 shape of the problem: one streaming pass over [H r] (L2/HBM), all flops in register-tiled FP64 FMA
+// Why it is the GPU shape of the problem: one streaming pass over [H r] (L2/HBM), all flops in register-tiled FP64 FMA
 // GEMM tiles spread over every SM, deterministic two-stage reduction, then ONE small factorisation — instead of
 // 154 x 3 sequential Householder steps. Multi-GPU needs no second-stage QR: Gram matrices add.
 #include "chol.cuh"

@@ -102,7 +102,7 @@ ovb_status ovb_create(const ovb_config *cfg, ovb_ctx **out) {
     const char *e4 = getenv("OVB_EKF_CHOL_DMMA");
     ctx->ekf_chol_dmma = e4 ? atoi(e4) : 1;
     const char *e5 = getenv("OVB_GRAM_CLUSTER");
-    ctx->gram_cluster = e5 ? atoi(e5) : 0; // measured slower on B200 (37 clusters of 4 do not co-schedule on 148 SMs: second wave), profiles/README.md
+    ctx->gram_cluster = e5 ? atoi(e5) : 0; // measured slower on H100 (config 2: compress 238 vs 190 us), profiles/README.md
   }
   CK(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
   ctx->own_stream = 1;
@@ -985,7 +985,7 @@ ovb_status ovb_msckf_replay(ovb_ctx *ctx, int steps, int flush_l2, float *ms_per
     return OVB_ERR_ARG;
   }
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-  const size_t flush_bytes = (size_t)256 << 20; // > 126 MB of L2
+  const size_t flush_bytes = (size_t)256 << 20; // five times the 50 MB L2 of an H100
   if (flush_l2 && !ctx->d_flush)
     OVB_CUDA_CHECK(ctx, cudaMalloc(&ctx->d_flush, flush_bytes));
   std::vector<cudaEvent_t> evs((size_t)steps * 6);

@@ -1,5 +1,5 @@
 """bench.py's reference arm runs on the host alone: check that it prints exactly ONE JSON line with the contract's keys.
-(The GPU arm needs a B200; its line is produced by the same code path for the shared keys.)"""
+(The GPU arm needs an H100; its line is produced by the same code path for the shared keys.)"""
 import json
 import os
 import subprocess

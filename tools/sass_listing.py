@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""profiles/sass_r02.txt: per-kernel opcode counts of the shipped libovb200.so (cuobjdump -sass) — the SASS evidence of the
+"""profiles/sass.txt: per-kernel opcode counts of the shipped libovb200.so (cuobjdump -sass) — the SASS evidence of the
 FP64 tensor-core path (DMMA), cp.async (LDGSTS), the hardware-seeded pivot rsqrt (MUFU.RSQ64H) and of the absence of
-tcgen05 / TMA opcodes (tcgen05 has no FP64 kind). Runs without a GPU."""
+wgmma / tensor-map TMA opcodes (wgmma has no FP64 kind). Runs without a GPU."""
 import collections
 import os
 import re
@@ -11,7 +11,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, "open_vins_b200", "libovb200.so")
 out = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
-WATCH = ["DMMA", "DFMA", "DMUL", "DADD", "MUFU.RSQ64H", "MUFU.RCP64H", "LDGSTS", "UBLKCP", "SYNCS", "SHFL", "BAR", "LDS", "STS", "UTMALDG", "UTCHMMA", "UTCQMMA", "UTCIMMA", "LDTM", "STTM"]
+WATCH = ["DMMA", "DFMA", "DMUL", "DADD", "MUFU.RSQ64H", "MUFU.RCP64H", "LDGSTS", "UBLKCP", "SYNCS", "SHFL", "BAR", "LDS", "STS", "UTMALDG", "HGMMA", "IGMMA", "QGMMA"]
 counts = collections.OrderedDict()
 fn = None
 for line in out.splitlines():
@@ -28,10 +28,10 @@ for line in out.splitlines():
                 counts[fn][w] += 1
                 break
 demangle = subprocess.run(["c++filt"], input="\n".join(counts.keys()), capture_output=True, text=True).stdout.splitlines()
-with open(os.path.join(ROOT, "profiles", "sass_r02.txt"), "w") as f:
-    f.write("# SASS opcode counts per kernel of open_vins_b200/libovb200.so (cuobjdump -sass, sm_100a), round 2; regenerate: python tools/sass_listing.py\n")
+with open(os.path.join(ROOT, "profiles", "sass.txt"), "w") as f:
+    f.write("# SASS opcode counts per kernel of open_vins_b200/libovb200.so (cuobjdump -sass, sm_90a); regenerate: python tools/sass_listing.py\n")
     f.write("# DMMA = mma.sync.m8n8k4.f64 (FP64 tensor-core path); LDGSTS = cp.async; MUFU.RSQ64H = rsqrt.approx.f64 pivot seed.\n")
-    f.write("# UBLKCP = cp.async.bulk (TMA engine, 1-D) + SYNCS = mbarrier ops: the packed Cholesky factor of k_cq_trsm. tcgen05 / tensor-map TMA opcodes\n# (UTC*MMA, UTMALDG, LDTM, STTM): none — tcgen05.mma has no FP64 kind, and every other operand tile here is\n")
+    f.write("# UBLKCP = cp.async.bulk (TMA engine, 1-D) + SYNCS = mbarrier ops: the packed Cholesky factor of k_cq_trsm. wgmma / tensor-map TMA opcodes\n# (HGMMA, IGMMA, QGMMA, UTMALDG): none — wgmma has no FP64 kind, and every other operand tile here is\n")
     f.write("# either register-resident or a few KB staged by cp.async (DESIGN.md §4).\n")
     for (fn, c), dm in zip(counts.items(), demangle):
         name = dm.split("(")[0]
@@ -40,4 +40,4 @@ with open(os.path.join(ROOT, "profiles", "sass_r02.txt"), "w") as f:
     for c in counts.values():
         tot.update(c)
     f.write("TOTAL " + " ".join(f"{k}={tot[k]}" for k in WATCH) + "\n")
-print(open(os.path.join(ROOT, "profiles", "sass_r02.txt")).read()[:3000])
+print(open(os.path.join(ROOT, "profiles", "sass.txt")).read()[:3000])

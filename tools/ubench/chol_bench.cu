@@ -1,5 +1,5 @@
 // Micro-benchmark: single-CTA blocked Cholesky variants (cycles by clock64), n = 154 (EKF) and n = 81 (chi2 gate).
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -I open_vins_b200/csrc -o tools/ubench/chol_bench tools/ubench/chol_bench.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I open_vins_b200/csrc -o tools/ubench/chol_bench tools/ubench/chol_bench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>

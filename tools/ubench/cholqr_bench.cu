@@ -1,5 +1,5 @@
 // cholqr_bench.cu — stand-alone timing of the CholeskyQR2 kernels (csrc/k_cholqr.cu) and of the DMMA latency/throughput
-// they are built on. Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 [-DCQ_PROBE] -o cholqr_bench cholqr_bench.cu
+// they are built on. Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 [-DCQ_PROBE] -o cholqr_bench cholqr_bench.cu
 #include "../../open_vins_b200/csrc/k_cholqr.cu"
 #include <cstdio>
 #include <vector>

@@ -1,8 +1,7 @@
 // diag8_bench.cu — what bounds the 8x8 pivot block of the tile Cholesky (csrc/chol_tiles.cuh)?
 //   * issue rate of independent FP64 FMAs from ONE warp (the pivot block is one warp's work)
-//   * the pivot block in the DMMA fragment layout (ct_diag8_frag). History on B200: every lane factoring the whole block in
-//     registers 2202 cycles; fragment layout with column j broadcast after scaling 1372 cycles; current form: see output
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o diag8_bench diag8_bench.cu
+//   * the pivot block in the DMMA fragment layout (ct_diag8_frag), in the form chol_tiles.cuh ships
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o diag8_bench diag8_bench.cu
 #include "../../open_vins_b200/csrc/chol_tiles.cuh"
 #include <cstdio>
 #include <vector>
