@@ -34,6 +34,7 @@ extern "C" {
 #define OVB_MAX_CAMS 8    /* cameras per rig (reference: StateOptions::num_cameras) */
 #define OVB_MAX_CLONES 48 /* clone poses in the sliding window incl. the newest */
 #define OVB_MAX_VARS (OVB_MAX_CLONES + 2 * OVB_MAX_CAMS) /* 6/6/8-wide state variables a feature can touch */
+#define OVB_MAX_MEAS_PER_FEAT (OVB_MAX_CAMS * OVB_MAX_CLONES) /* measurements of one feature track: every camera in every clone */
 #define OVB_CHI2_TABLE_LEN 2048
 
 /* ---- status codes (replace the reference's std::exit paths, state/StateHelper.cpp:103-113,172-182) ---- */
@@ -161,7 +162,10 @@ typedef struct {
  * Measurements at non-clone times must already be removed (Feature::clean_old_measurements, UpdaterMSCKF.cpp:79).
  * cam_keys lists, per feature, the camera keys of feat->timestamps in visit order INCLUDING cameras whose list is
  * empty after cleaning (they still contribute calibration columns, update/UpdaterHelper.cpp:204-222); pass NULL to
- * derive the list from the measurements themselves. */
+ * derive the list from the measurements themselves.
+ * A feature has at most OVB_MAX_MEAS_PER_FEAT (= OVB_MAX_CAMS * OVB_MAX_CLONES = 384) measurements: one per camera and
+ * clone pose. A longer track makes the whole call return OVB_ERR_CAPACITY. Tracks of any length up to the limit may be
+ * mixed in one batch; each runs on the per-feature kernel layout it fits. */
 typedef struct {
   int n_feats;
   int n_meas;

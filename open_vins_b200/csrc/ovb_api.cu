@@ -166,7 +166,7 @@ ovb_status ovb_create(const ovb_config *cfg, ovb_ctx **out) {
   CK(cudaMalloc(&ctx->d_S, sizeof(double) * (size_t)(ms + 1) * ms));
   CK(cudaMalloc(&ctx->d_Y, sizeof(double) * (size_t)ms * ms));
   CK(cudaMalloc(&ctx->d_w, sizeof(double) * (size_t)ms * 4));
-  ctx->scratch_per_cta = (size_t)(2 * OVB_MAX_MEAS_PER_FEAT + 1) * (2 * OVB_MAX_MEAS_PER_FEAT + 1);
+  ctx->scratch_per_cta = (size_t)(2 * OVB_BIG_MAX_MEAS + 1) * (2 * OVB_BIG_MAX_MEAS + 1);
   ctx->scratch_ctas = 2 * ctx->sm_count;
   CK(cudaMalloc(&ctx->d_scratch, sizeof(double) * ctx->scratch_per_cta * ctx->scratch_ctas));
   ctx->dump_cap = 0;
@@ -188,7 +188,7 @@ void ovb_destroy(ovb_ctx *ctx) {
     cudaStreamSynchronize(ctx->stream);
   void *dev[] = {ctx->P[0],   ctx->P[1], ctx->d_arena, ctx->d_cc, ctx->d_feat_order, ctx->d_info, ctx->d_chi2_table, ctx->d_Hs, ctx->d_W[0],
                  ctx->d_W[1], ctx->d_R,  ctx->d_R2,    ctx->d_M,  ctx->d_S,          ctx->d_Y,    ctx->d_w,          ctx->d_scratch,
-                 ctx->d_dump, ctx->P_snap, ctx->d_flush, ctx->d_Gpart, ctx->d_G, ctx->d_cqw};
+                 ctx->d_long, ctx->d_dump, ctx->P_snap, ctx->d_flush, ctx->d_Gpart, ctx->d_G, ctx->d_cqw};
   for (void *p : dev)
     if (p)
       cudaFree(p);
@@ -348,14 +348,15 @@ ovb_status ovb_cov_propagate(ovb_ctx *ctx, int new_off, int p, const int *old_of
 
 // ------------------------------------------------------------------------------------------------ marshalling
 struct Packed {
-  int n_feats, n_meas, max_M, m_total, ldH, n_all;
+  int n_feats, n_meas, m_total, ldH, n_all;
   BlobView bv;
 };
 
 // lm != nullptr: SLAM batch — every feature brings its landmark (a 3-wide state variable that becomes one more slot),
 // rows are NOT nullspace-projected (2M per feature instead of 2M-3), values/anchors come from the landmark.
+// per_feature: the call will launch the per-feature kernel (everything but ovb_triangulate), so its scratch is reserved.
 static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_batch *fb, const ovb_opts *op, const ovb_feat_out *given,
-                              Packed *pk, const ovb_landmarks *lm = nullptr) {
+                              Packed *pk, const ovb_landmarks *lm = nullptr, bool per_feature = true) {
   if (!fr || !fb || !op)
     return OVB_ERR_ARG;
   if (lm && (!lm->lm_off || !lm->value || !lm->value_fej))
@@ -467,7 +468,7 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
   }
   unsigned char *hkeys = hb + o_keys;
   size_t nkeys = 0;
-  int row = 0, maxM = 0;
+  int row = 0;
   for (int f = 0; f < F; f++) {
     DevFeat &d = ctx->h_feat[f];
     d.m0 = fb->meas_off[f];
@@ -479,7 +480,6 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
       snprintf(ctx->err, sizeof(ctx->err), "feature %d has %d measurements (max %d)", f, Mf, OVB_MAX_MEAS_PER_FEAT);
       return OVB_ERR_CAPACITY;
     }
-    maxM = std::max(maxM, Mf);
     d.row0 = row;
     if (lm)
       row += lm_single ? (Mf >= 2 ? 2 * Mf - 2 : 0) : 2 * Mf; // UpdaterSLAM.cpp:344-387: all 2M rows kept (SINGLE: 2 projected out)
@@ -583,13 +583,17 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
   }
   pk->n_feats = F;
   pk->n_meas = M;
-  pk->max_M = maxM;
   pk->m_total = row;
   pk->n_all = col;
   pk->ldH = (int)align_up((size_t)col + 1, 4);
   if ((size_t)std::max(row, col) * pk->ldH > ctx->Hs_cap || row > ctx->max_rows) {
     snprintf(ctx->err, sizeof(ctx->err), "stacked system %d x %d exceeds the reserved staging matrix", row, pk->ldH);
     return OVB_ERR_CAPACITY;
+  }
+  if (per_feature) { // long tracks: scratch of the per-feature kernel's long-track path
+    ovb_status rs = feature_scratch_reserve(ctx, F, lm != nullptr);
+    if (rs != OVB_OK)
+      return rs;
   }
   pk->bv.cam = ctx->d_blob + o_cam;
   pk->bv.clone = (const uint16_t *)(ctx->d_blob + o_clone);
@@ -637,7 +641,7 @@ ovb_status ovb_triangulate(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_
   int saveN = ctx->N;
   if (ctx->N == 0)
     ctx->N = ctx->cfg.max_state; // offsets are not dereferenced by this stage
-  ovb_status st = pack_inputs(ctx, frame, feats, opts, nullptr, &pk);
+  ovb_status st = pack_inputs(ctx, frame, feats, opts, nullptr, &pk, nullptr, false);
   ctx->N = saveN;
   if (st != OVB_OK)
     return st;
@@ -683,7 +687,7 @@ ovb_status ovb_feature_jacobians(ovb_ctx *ctx, const ovb_frame *frame, const ovb
     }
     ctx->dump_rows = rows;
     OVB_CUDA_CHECK(ctx, cudaMemsetAsync(ctx->d_dump, 0, sizeof(double) * need, ctx->stream));
-    launch_feature_system(ctx, F, pk.bv, pk.ldH, 1, pk.max_M);
+    launch_feature_system(ctx, F, pk.bv, pk.ldH, 1);
     OVB_CUDA_CHECK(ctx, cudaGetLastError());
     std::vector<double> host(need);
     OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(host.data(), ctx->d_dump, sizeof(double) * need, cudaMemcpyDeviceToHost, ctx->stream));
@@ -704,7 +708,7 @@ ovb_status ovb_feature_jacobians(ovb_ctx *ctx, const ovb_frame *frame, const ovb
     }
     return OVB_OK;
   }
-  launch_feature_system(ctx, F, pk.bv, pk.ldH, 0, pk.max_M);
+  launch_feature_system(ctx, F, pk.bv, pk.ldH, 0);
   OVB_CUDA_CHECK(ctx, cudaGetLastError());
   std::vector<double> host((size_t)pk.m_total * pk.ldH);
   if (pk.m_total > 0)
@@ -848,7 +852,7 @@ static int compress_system(ovb_ctx *ctx, int mode, double *A, int m, int n, int 
 // ev (optional): ev[1] after triangulation, ev[2] after the per-feature systems, ev[3] after the column map, ev[4] after
 // compression, ev[5] after the EKF update. Returns the row count handed to the EKF update.
 // slam: UpdaterSLAM::update — landmarks come from the state (no triangulation), rows are kept unprojected and whitened.
-static int enqueue_update(ovb_ctx *ctx, int F, BlobView bv, int ldH, int max_M, int m_total, int n_all, int col_order, cudaEvent_t *ev,
+static int enqueue_update(ovb_ctx *ctx, int F, BlobView bv, int ldH, int m_total, int n_all, int col_order, cudaEvent_t *ev,
                           bool slam = false) {
   const int N = ctx->N;
   ctx->n_launch = 0;
@@ -862,7 +866,7 @@ static int enqueue_update(ovb_ctx *ctx, int F, BlobView bv, int ldH, int max_M, 
   ctx->n_launch += 1; // column map (the per-feature kernel counts its own launches: one, or one per size class)
   if (ev)
     cudaEventRecord(ev[1], ctx->stream);
-  launch_feature_system(ctx, F, bv, ldH, slam ? 2 : 0, max_M);
+  launch_feature_system(ctx, F, bv, ldH, slam ? 2 : 0);
   if (ev)
     cudaEventRecord(ev[2], ctx->stream);
   // the column bookkeeping (a single serial CTA) only feeds the re-ordering and the EKF update: it runs on the side
@@ -999,7 +1003,7 @@ ovb_status ovb_msckf_replay(ovb_ctx *ctx, int steps, int flush_l2, float *ms_per
     cudaMemcpyAsync(ctx->P[ctx->cur], ctx->P_snap, Pbytes, cudaMemcpyDeviceToDevice, ctx->stream);
     cudaEvent_t *ev = &evs[(size_t)s * 6];
     cudaEventRecord(ev[0], ctx->stream);
-    enqueue_update(ctx, ctx->last_n_feats, ctx->last_bv, ctx->last_ldH, ctx->last_max_M, ctx->last_m_total, ctx->last_n_all, ctx->last_col_order,
+    enqueue_update(ctx, ctx->last_n_feats, ctx->last_bv, ctx->last_ldH, ctx->last_m_total, ctx->last_n_all, ctx->last_col_order,
                    ev);
   }
   OVB_CUDA_CHECK(ctx, cudaGetLastError());
@@ -1054,14 +1058,13 @@ ovb_status ovb_msckf_update(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat
                                         ctx->stream));
     ctx->last_pk_valid = 1;
     ctx->last_n_feats = pk.n_feats;
-    ctx->last_max_M = pk.max_M;
     ctx->last_m_total = pk.m_total;
     ctx->last_ldH = pk.ldH;
     ctx->last_n_all = pk.n_all;
     ctx->last_bv = pk.bv;
     ctx->last_col_order = opts->col_order;
   }
-  const int r = enqueue_update(ctx, pk.n_feats, pk.bv, pk.ldH, pk.max_M, pk.m_total, pk.n_all, opts->col_order, ctx->ev);
+  const int r = enqueue_update(ctx, pk.n_feats, pk.bv, pk.ldH, pk.m_total, pk.n_all, opts->col_order, ctx->ev);
   OVB_CUDA_CHECK(ctx, cudaGetLastError());
   OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_feat, ctx->d_feat, sizeof(DevFeat) * (size_t)F, cudaMemcpyDeviceToHost, ctx->stream));
   OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_info, ctx->d_info, ctx->info_bytes + sizeof(double) * (size_t)N, cudaMemcpyDeviceToHost,
@@ -1137,7 +1140,7 @@ ovb_status ovb_slam_update(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_
     return st;
   const int F = pk.n_feats;
   ctx->last_pk_valid = 0; // the replay path re-runs MSCKF updates only
-  const int r = enqueue_update(ctx, pk.n_feats, pk.bv, pk.ldH, pk.max_M, pk.m_total, pk.n_all, opts->col_order, ctx->ev, true);
+  const int r = enqueue_update(ctx, pk.n_feats, pk.bv, pk.ldH, pk.m_total, pk.n_all, opts->col_order, ctx->ev, true);
   OVB_CUDA_CHECK(ctx, cudaGetLastError());
   OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_feat, ctx->d_feat, sizeof(DevFeat) * (size_t)F, cudaMemcpyDeviceToHost, ctx->stream));
   OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_info, ctx->d_info, ctx->info_bytes + sizeof(double) * (size_t)N, cudaMemcpyDeviceToHost,
@@ -1294,7 +1297,7 @@ ovb_status ovb_msckf_shard_compress(ovb_ctx *ctx, const ovb_frame *frame, const 
   ctx->n_launch_tsqr_level = 0;
   launch_cam_poses(ctx);
   launch_triangulate(ctx, pk.n_feats, pk.bv);
-  launch_feature_system(ctx, pk.n_feats, pk.bv, pk.ldH, 0, pk.max_M);
+  launch_feature_system(ctx, pk.n_feats, pk.bv, pk.ldH, 0);
   launch_column_map(ctx, pk.n_feats, pk.bv);
   ctx->n_launch += 3; // cam poses, triangulate, column map (+ the per-feature kernel's own count)
   if (pk.m_total > 0)

@@ -4,7 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#define OVB_MAX_MEAS_PER_FEAT 128 // K*C of config 4 is 124 (SURVEY.md §8 sizes table)
+// OVB_MAX_MEAS_PER_FEAT (include/ovb200.h): 384 = every camera in every clone pose
+#define OVB_BIG_MAX_MEAS 128      // longest track of the per-feature kernel's BIG path: d_scratch is sized for it at ovb_create
 #define OVB_MAX_COLS 512          // >= 6*OVB_MAX_CLONES + 14*OVB_MAX_CAMS; also the widest H of ovb_ekf_update (config 5: n = 500)
 #define OVB_NB 16                 // TSQR panel width
 #define OVB_CR 256                // TSQR rows per chunk
@@ -131,9 +132,11 @@ struct ovb_ctx {
   double *d_Y;   // EKF: M L^-T
   double *d_w;   // EKF: L^-1 z
   double *d_dx;
-  double *d_scratch; // per-CTA scratch for large features in the gate kernel
+  double *d_scratch; // per-CTA scratch for large features in the gate kernel (BIG path, up to OVB_BIG_MAX_MEAS measurements)
   size_t scratch_per_cta;
   int scratch_ctas;
+  double *d_long;    // per-CTA scratch of the long-track path (feature_scratch_reserve: sized by the call's tracks, grown on demand)
+  size_t long_cap;   // doubles
   double *d_dump; // debug dumps for ovb_feature_jacobians
   size_t dump_cap;
   int dump_rows;
@@ -150,7 +153,7 @@ struct ovb_ctx {
   double host_us[4]; // host wall clock of the last ovb_msckf_update: marshalling + H2D enqueue, kernel enqueue, wait, result unpack
   // replay of the last update on device-resident inputs (bench: `value` leg; see ovb_msckf_replay)
   int replay_enabled, last_pk_valid;
-  int last_n_feats, last_max_M, last_m_total, last_ldH, last_n_all, last_col_order;
+  int last_n_feats, last_m_total, last_ldH, last_n_all, last_col_order;
   BlobView last_bv;
   double *P_snap;
   void *d_flush;
@@ -182,7 +185,10 @@ void launch_cam_poses(ovb_ctx *ctx);
 void launch_triangulate(ovb_ctx *ctx, int n_feats, BlobView bv);
 // mode 0: normal (write post-nullspace rows to Hs, gate on chi²); mode 1: dump pre-nullspace dense rows to d_dump
 // mode 2: like 0 but features keep the status/p_FinG given (no triangulation ran) — used by ovb_feature_jacobians
-void launch_feature_system(ovb_ctx *ctx, int n_feats, BlobView bv, int ldH, int mode, int max_M);
+// Every track runs on the path it fits (shared-memory tile, BIG, or long-track; see k_feature.cu).
+void launch_feature_system(ovb_ctx *ctx, int n_feats, BlobView bv, int ldH, int mode);
+// grow the long-track scratch for the tracks of the packed batch (h_feat); slam: the batch is a SLAM update
+ovb_status feature_scratch_reserve(ovb_ctx *ctx, int n_feats, bool slam);
 void launch_column_map(ovb_ctx *ctx, int n_feats, BlobView bv, int rows_drop = 3);
 // TSQR of A [m x (n+1)] (last column = residual) in place; R (n x (n+1), diag>=0) to Rout with leading dimension ldR
 void launch_tsqr(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR);

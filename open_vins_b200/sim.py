@@ -15,7 +15,7 @@ import numpy as np
 
 from .capi import FeatArrays, FrameArrays
 
-# config/rpng_sim/kalibr_imucam_chain.yaml (T_imu_cam = [R_CtoI, p_CinI]); cams 0..3
+# config/rpng_sim/kalibr_imucam_chain.yaml (T_imu_cam = [R_CtoI, p_CinI]); cams 0..3 (4..7: _cam_extrinsic)
 _T_IMU_CAM = [
     [[0.0148655429818, -0.999880929698, 0.00414029679422, -0.0216401454975],
      [0.999557249008, 0.0149672133247, 0.025715529948, -0.064676986768],
@@ -36,6 +36,17 @@ _INTR = [
     [458.654, 457.296, 367.215, 248.375, -0.28340811, 0.07395907, 0.00019359, 1.76187114e-05],
     [457.587, 456.134, 379.999, 255.238, -0.28368365, 0.07451284, -0.00010473, -3.55590700e-05],
 ]
+def _cam_extrinsic(k):
+    """T_imu_cam of camera k: cameras 0..3 are the rpng_sim chain; cameras 4..7 repeat cameras 0..3 on a second rig
+    level, 0.3 m below and yawed by 5 degrees about the IMU z axis (deterministic, no random draws: the generated cases
+    of n_cams <= 4 stay bit-identical)."""
+    T = np.array(_T_IMU_CAM[k % 4])
+    if k < 4:
+        return T
+    Rz = exp_so3(np.array([0.0, 0.0, np.deg2rad(5.0)]))
+    return np.hstack([Rz @ T[:, :3], (Rz @ T[:, 3] + np.array([0.0, 0.0, -0.3]))[:, None]])
+
+
 # a mild equidistant set for the fisheye model tests
 _INTR_EQUI = [190.978, 190.973, 254.93, 256.897, 0.0034, 0.0007, -0.0020, 0.0002]
 
@@ -192,9 +203,11 @@ def make_update_case(n_feats=50, n_clones=12, n_cams=1, seed=0, calib_ext=False,
         R_true.append(R)
         p_true.append(p)
     R_true, p_true = np.array(R_true), np.array(p_true)
-    camR_true = np.array([np.array(_T_IMU_CAM[k])[:, :3].T for k in range(n_cams)])  # R_ItoC = R_CtoI'
-    camp_true = np.array([-camR_true[k] @ np.array(_T_IMU_CAM[k])[:, 3] for k in range(n_cams)])  # p_IinC
-    intr_true = np.array([_INTR[k] if cam_model == 0 else _INTR_EQUI for k in range(n_cams)], dtype=np.float64)
+    if not 1 <= n_cams <= 8:
+        raise ValueError(f"n_cams={n_cams}: the generator has 8 cameras")
+    camR_true = np.array([_cam_extrinsic(k)[:, :3].T for k in range(n_cams)])  # R_ItoC = R_CtoI'
+    camp_true = np.array([-camR_true[k] @ _cam_extrinsic(k)[:, 3] for k in range(n_cams)])  # p_IinC
+    intr_true = np.array([_INTR[k % 4] if cam_model == 0 else _INTR_EQUI for k in range(n_cams)], dtype=np.float64)
     # ---- prior covariance: D (0.6 I + 0.4 U U'/k) D, SPD with cross-correlations
     sig = lay.sigmas()
     k = 12
