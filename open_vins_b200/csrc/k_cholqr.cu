@@ -5,9 +5,13 @@
 //
 //   pass 1   G1 = [H r]'[H r]                      k_cq_gram (DMMA, row slabs over all SMs) + k_cq_reduce (fixed order)
 //            R1'R1 = G1 + s1 I                      k_cq_chol_gram (one CTA, tile-packed in shared memory: chol_tiles.cuh)
-//            Q1 = [H r] R1^-1   (in place)          k_cq_trsm (row groups in registers, right-looking, DMMA)
-//   pass 2   G2 = Q1'Q1,  R2'R2 = G2 + s2 I         the same two kernels
+//   pass 2   G2 = Q1'Q1,  Q1 = [H r] R1^-1          k_cq_solve_gram: each slab's rows solved in shared memory (k_cq_trsm's
+//                                                   row solve) and fed straight to k_cq_gram's k-steps; only a slab's last
+//                                                   rows past the buffer pass through a small scratch, the rest of Q1 never
+//                                                   reaches global memory, and [H r] is left as it was. Then k_cq_reduce.
+//            R2'R2 = G2 + s2 I                      k_cq_chol_gram
 //            [R z] = rows 0..n-1 of R2 R1           k_cq_trmm
+// Systems wider than CQ_MAXN take the blocked path (cq_compress_wide), which overwrites [H r] with Q1.
 //
 // Why two passes are enough for the filter (DESIGN.md §4): StateHelper::EKFUpdate (state/StateHelper.cpp:116-197) sees
 // the compressed system only through R'R = H'H and R'z = H'r. With Q1 = A R1^-1 computed by row-wise backward-stable
@@ -89,6 +93,50 @@ __device__ __forceinline__ bool cq_tile_origin(int blk, int w, int BW, int nblk_
   return true;
 }
 
+// Rows rc..rc+nrows-1 of A into buf (row-major, `pitch` doubles): columns [cI0, cI0+WI) and, nrng == 2, [cJ0, cJ0+WI)
+// after them, by 16-byte cp.async (NT threads, one commit group) with zero fill for rows >= r1 and columns >= nt.
+template <int NT>
+__device__ __forceinline__ void cq_issue_rows(double *buf, int pitch, const double *__restrict__ A, int ldA, int rc, int nrows, int r1, int nt, int cI0, int cJ0,
+                                              int WI, int nrng) {
+  const int units_per_row = nrng * WI / 2;
+  for (int e = threadIdx.x; e < nrows * units_per_row; e += NT) {
+    const int k = e / units_per_row, u = e - k * units_per_row;
+    const int r = rc + k;
+    const int dcol = 2 * u, col = (dcol < WI) ? cI0 + dcol : cJ0 + (dcol - WI);
+    unsigned bytes = 0;
+    if (r < r1)
+      bytes = (col + 1 < nt) ? 16u : (col < nt ? 8u : 0u);
+    const double *src = bytes ? (A + (size_t)r * ldA + col) : A;
+    cpa16(s_u32(buf + (size_t)k * pitch + dcol), src, bytes);
+  }
+  cpa_commit();
+}
+
+// acc += one k-step (4 staged rows at `row0`) of one warp tile. Both Gram kernels accumulate through this, k-step by k-step
+// in row order, so their partials over the same rows agree bit for bit. Both DMMA operands are the fragment
+// X[lane&3][c0 + (lane>>2)] of the staged rows, at c0 = offI (row side) and offJ (column side); same: offI == offJ.
+__device__ __forceinline__ void cq_gram_kstep(double (&acc)[4][4][2], const double *row0, int pitch, int offI, int offJ, bool same, int g, int q) {
+  const double *row = row0 + (size_t)q * pitch + g;
+  double fa[4], fb[4];
+#pragma unroll
+  for (int b = 0; b < 4; b++)
+    fa[b] = row[offI + 8 * b];
+  if (same) {
+#pragma unroll
+    for (int b = 0; b < 4; b++)
+      fb[b] = fa[b];
+  } else {
+#pragma unroll
+    for (int b = 0; b < 4; b++)
+      fb[b] = row[offJ + 8 * b];
+  }
+#pragma unroll
+  for (int a = 0; a < 4; a++)
+#pragma unroll
+    for (int b = 0; b < 4; b++)
+      dmma(acc[a][b][0], acc[a][b][1], fa[a], fb[b]);
+}
+
 } // namespace
 
 // ------------------------------------------------------------------------------------------------------------ Gram
@@ -117,7 +165,6 @@ __global__ void __launch_bounds__(CQ_GRAM_T) k_cq_gram(const double *__restrict_
   const int cI0 = bI * WI, cJ0 = bJ * WI;
   const int r0 = blockIdx.y * slab_rows, r1 = min(m, r0 + slab_rows);
   const int nchunks = (r1 > r0) ? (r1 - r0 + CQ_KB - 1) / CQ_KB : 0;
-  const int units_per_row = nrng * WI / 2;
   double acc[4][4][2];
 #pragma unroll
   for (int a = 0; a < 4; a++)
@@ -125,28 +172,7 @@ __global__ void __launch_bounds__(CQ_GRAM_T) k_cq_gram(const double *__restrict_
     for (int b = 0; b < 4; b++)
       acc[a][b][0] = acc[a][b][1] = 0.0;
 
-  auto issue = [&](int c) {
-    double *buf = gsm + (size_t)(c & 1) * CQ_KB * pitch;
-    const int rc = r0 + c * CQ_KB;
-    for (int e = tid; e < CQ_KB * units_per_row; e += CQ_GRAM_T) {
-      const int k = e / units_per_row, u = e - k * units_per_row;
-      const int r = rc + k;
-      int col, dcol;
-      if (2 * u < WI) {
-        col = cI0 + 2 * u;
-        dcol = 2 * u;
-      } else {
-        col = cJ0 + (2 * u - WI);
-        dcol = 2 * u;
-      }
-      unsigned bytes = 0;
-      if (r < r1)
-        bytes = (col + 1 < nt) ? 16u : (col < nt ? 8u : 0u);
-      const double *src = bytes ? (A + (size_t)r * ldA + col) : A;
-      cpa16(s_u32(buf + (size_t)k * pitch + dcol), src, bytes);
-    }
-    cpa_commit();
-  };
+  auto issue = [&](int c) { cq_issue_rows<CQ_GRAM_T>(gsm + (size_t)(c & 1) * CQ_KB * pitch, pitch, A, ldA, r0 + c * CQ_KB, CQ_KB, r1, nt, cI0, cJ0, WI, nrng); };
   if (nchunks > 0)
     issue(0);
   for (int c = 0; c < nchunks; c++) {
@@ -160,27 +186,8 @@ __global__ void __launch_bounds__(CQ_GRAM_T) k_cq_gram(const double *__restrict_
     if (active) {
       const double *buf = gsm + (size_t)(c & 1) * CQ_KB * pitch;
 #pragma unroll
-      for (int ks = 0; ks < CQ_KB / 4; ks++) {
-        const double *row = buf + (size_t)(4 * ks + q) * pitch + g;
-        double fa[4], fb[4];
-#pragma unroll
-        for (int b = 0; b < 4; b++)
-          fa[b] = row[offI + 8 * b];
-        if (diag && offI == offJ) {
-#pragma unroll
-          for (int b = 0; b < 4; b++)
-            fb[b] = fa[b];
-        } else {
-#pragma unroll
-          for (int b = 0; b < 4; b++)
-            fb[b] = row[offJ + 8 * b];
-        }
-#pragma unroll
-        for (int a = 0; a < 4; a++)
-#pragma unroll
-          for (int b = 0; b < 4; b++)
-            dmma(acc[a][b][0], acc[a][b][1], fa[a], fb[b]);
-      }
+      for (int ks = 0; ks < CQ_KB / 4; ks++)
+        cq_gram_kstep(acc, buf + (size_t)4 * ks * pitch, pitch, offI, offJ, diag && offI == offJ, g, q);
     }
     __syncthreads();
   }
@@ -568,19 +575,12 @@ __device__ __forceinline__ void cq_trsm_store(const double (&acc)[NH][2], double
   }
 }
 
-// NH1 + NH2 >= ceil(nt / 8); NH2 == 0: single half
-template <int NH1, int NH2>
-__global__ void __launch_bounds__(CQ_TRSM_T) k_cq_trsm(double *__restrict__ A, int ldA, int m, int nt, const double *__restrict__ Lpk) {
-  OVB_PDL_ENTER();
-  extern __shared__ __align__(16) double tsm[];
-  double *Lt = tsm;
-  double *Ri = tsm + CQ_PK_INV;
-  double *Xs = tsm + CQ_PK_DOUBLES; // per warp: first-half A-operand fragments [NH1][2][32]
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, g = lane >> 2, q = lane & 3;
-  const int NB = (nt + 7) >> 3;
-  constexpr int NBP = NH1 + NH2; // padded block count: tiles past NB are zero, their reciprocal pivots 1
-  // the packed factor (up to 106 KB, contiguous) arrives as two bulk copies (TMA engine, SASS UBLKCP) signalled on an
-  // mbarrier: one instruction issues them, nobody spends issue slots or registers on the transfer
+// The packed factor into shared memory, padded to NBP blocks (tiles past NB zero, their reciprocal pivots 1). It (up to
+// 106 KB, contiguous) arrives as two bulk copies (TMA engine, SASS UBLKCP) signalled on an mbarrier: one instruction issues
+// them, nobody spends issue slots or registers on the transfer. Ends with a barrier; NT = threads of the CTA.
+template <int NBP, int NT>
+__device__ __forceinline__ void cq_fetch_factor(double *Lt, double *Ri, const double *__restrict__ Lpk, int NB) {
+  const int tid = threadIdx.x;
   __shared__ __align__(8) unsigned long long l_bar;
   const unsigned bar = s_u32(&l_bar);
   if (tid == 0) {
@@ -597,13 +597,25 @@ __global__ void __launch_bounds__(CQ_TRSM_T) k_cq_trsm(double *__restrict__ A, i
                  "r"(bar)
                  : "memory");
   }
-  for (int e = tri(NB) * 64 + tid; e < tri(NBP) * 64; e += CQ_TRSM_T)
+  for (int e = tri(NB) * 64 + tid; e < tri(NBP) * 64; e += NT)
     Lt[e] = 0.0;
-  for (int e = NB * 8 + tid; e < NBP * 8; e += CQ_TRSM_T)
+  for (int e = NB * 8 + tid; e < NBP * 8; e += NT)
     Ri[e] = 1.0;
   asm volatile("{\n\t.reg .pred p;\n\tCQ_LWAIT:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], 0;\n\t@p bra CQ_LDONE;\n\tbra CQ_LWAIT;\n\tCQ_LDONE:\n\t}" ::"r"(bar)
                : "memory");
   __syncthreads();
+}
+
+// NH1 + NH2 >= ceil(nt / 8); NH2 == 0: single half
+template <int NH1, int NH2>
+__global__ void __launch_bounds__(CQ_TRSM_T) k_cq_trsm(double *__restrict__ A, int ldA, int m, int nt, const double *__restrict__ Lpk) {
+  OVB_PDL_ENTER();
+  extern __shared__ __align__(16) double tsm[];
+  double *Lt = tsm;
+  double *Ri = tsm + CQ_PK_INV;
+  double *Xs = tsm + CQ_PK_DOUBLES; // per warp: first-half A-operand fragments [NH1][2][32]
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, g = lane >> 2, q = lane & 3;
+  cq_fetch_factor<NH1 + NH2, CQ_TRSM_T>(Lt, Ri, Lpk, (nt + 7) >> 3);
   double *xs = Xs + (size_t)wid * (CQ_TRSM_NH * 2 * 32);
   const int ngroups = (m + 7) >> 3;
   // row groups are dealt round-robin over the CTAs first (warp w of CTA b takes group b + w * gridDim.x): a short matrix puts
@@ -670,6 +682,173 @@ static void cq_launch_trsm(ovb_ctx *ctx, int ctas, double *A, int ldA, int m, in
     ovb_launch(ctx, k_cq_trsm<10, 5>, dim3(ctas), dim3(CQ_TRSM_T), smem, A, ldA, m, nt, Lpk);
   else
     ovb_launch(ctx, k_cq_trsm<10, 10>, dim3(ctas), dim3(CQ_TRSM_T), smem, A, ldA, m, nt, Lpk);
+}
+
+// ------------------------------------------------------------------------------------------------------------ pass 2: solve + Gram
+// G2 = Q1'Q1 without Q1 in global memory: the Gram partials of pass 2 straight from A and the packed R1. One CTA per Gram
+// slab (pass 1's slabs), CQ_GRAM_T threads, R1 in shared memory as k_cq_trsm holds it. The slab is taken in rounds
+// through a shared buffer of `cb` rows, staged as k_cq_gram stages its rows (cp.async, row-major, zero fill past nt and
+// past the slab). When the slab's last rows exceed the buffer but not one 8-row group per warp, that last round splits:
+// its first rows (a whole number of row groups) go through the buffer, the rest through a per-slab scratch in global
+// memory laid out alike, so every row group of the round solves at once:
+//   solve   warp w solves rows 8w..8w+7 of the round with k_cq_trsm's row solve (per-row arithmetic unchanged), in place
+//           in the buffer or the scratch; the second half takes its A-operands from the solved first half there
+//   Gram    the tile warps run k_cq_gram's k-steps over the buffer, then over the scratch rows
+// Same slabs, same k-step order, zero rows contributing exact zeros: the partials are bit for bit those k_cq_gram forms
+// from a stored Q1, and A is left as it was. Between rounds each tile warp parks its accumulators in its own Gpart slot
+// (exact), so neither phase carries the other's registers. A buffer row holds all 8*NBP solved columns (at least the
+// BW*32 the Gram reads), pitch = 4 mod 16 for conflict-free fragment loads; the padding columns past nt are solved along
+// (zeros against a factor that is zero there) and only reach Gram entries past nt, which k_cq_reduce drops. Next to the
+// 107 KB factor the buffer holds 92 rows at 155 columns: config 2's 100-row slabs are one split round (88 + 12 rows)
+// instead of a 92-row round followed by a second solve of the last 8 rows.
+#define CQ_SG_SMEM (226 * 1024) // dynamic shared memory of k_cq_solve_gram, at most (sm_90 opt-in limit 227 KB, static part included)
+
+__host__ __device__ __forceinline__ int cq_sg_pitch(int BW, int NBP) {
+  const int w = (8 * NBP > 32 * BW) ? 8 * NBP : 32 * BW;
+  return ((w + 15) & ~15) + 4;
+}
+
+// one warp's 8-row group solved in place: xrow = the lane's row (8*NBP columns, zero past nt), k_cq_trsm's row solve; the
+// second half takes its A-operands from the solved first half in the row. Lanes with !row_ok (past the rows to solve)
+// load zeros and store nothing; their xrow must still be a row of the warp's group.
+template <int NH1, int NH2>
+__device__ __forceinline__ void cq_solve_group(double *xrow, bool row_ok, const double *Lt, const double *Ri, int lane) {
+  constexpr int NBP = NH1 + NH2;
+  const int g = lane >> 2, q = lane & 3;
+  {
+    double acc[NH1][2];
+    cq_trsm_load<NH1>(acc, xrow, row_ok, 0, 8 * NBP, q);
+    cq_trsm_half<NH1>(acc, 0, Lt, Ri, nullptr, lane);
+    cq_trsm_store<NH1>(acc, xrow, row_ok, 0, 8 * NBP, q);
+  }
+  if constexpr (NH2 > 0) {
+    double acc[NH2][2];
+    __syncwarp();
+    cq_trsm_load<NH2>(acc, xrow, row_ok, NH1, 8 * NBP, q);
+    // A[:, half 2] -= X[:, half 1] R[half 1, half 2]; the A-operand of row g, column 8jb + 4ks + q is the solved X, negated
+#pragma unroll 2
+    for (int jb = 0; jb < NH1; jb++) {
+      const double af0 = -xrow[8 * jb + q], af1 = -xrow[8 * jb + 4 + q];
+#pragma unroll
+      for (int j = 0; j < NH2; j++) {
+        const double *lf = Lt + (size_t)(tri(NH1 + j) + jb) * 64 + g * 8 + q;
+        dmma(acc[j][0], acc[j][1], af0, lf[0]);
+        dmma(acc[j][0], acc[j][1], af1, lf[4]);
+      }
+    }
+    cq_trsm_half<NH2>(acc, NH1, Lt, Ri, nullptr, lane);
+    cq_trsm_store<NH2>(acc, xrow, row_ok, NH1, 8 * NBP, q);
+  }
+}
+
+template <int NH1, int NH2>
+__global__ void __launch_bounds__(CQ_GRAM_T) k_cq_solve_gram(const double *__restrict__ A, int ldA, int m, int nt, const double *__restrict__ Lpk, int slab_rows,
+                                                            int cb, int ntail_max, int BW, double *__restrict__ Gpart, double *__restrict__ Qtail) {
+  OVB_PDL_ENTER();
+  extern __shared__ __align__(16) double ssm[];
+  double *Lt = ssm;
+  double *Ri = ssm + CQ_PK_INV;
+  double *X = ssm + CQ_PK_DOUBLES; // buffer [cb][pitch]
+  constexpr int NBP = NH1 + NH2;
+  const int pitch = cq_sg_pitch(BW, NBP);
+  const int r0 = blockIdx.x * slab_rows, r1 = min(m, r0 + slab_rows);
+  double *tail = Qtail + (size_t)blockIdx.x * ntail_max * pitch;
+  // the last round splits when its rows exceed the buffer but not one row group per warp
+  auto split_at = [&](int rc) { return r1 - rc > cb && r1 - rc <= 8 * (CQ_GRAM_T / 32); };
+  // rows the buffer takes in the round at rc (a partial k-step is padded with zero rows)
+  auto nbuf_at = [&](int rc) { return split_at(rc) ? cb & ~7 : min(cb, (r1 - rc + 3) & ~3); };
+  // the first round's rows are in flight while the factor arrives
+  if (r0 < r1)
+    cq_issue_rows<CQ_GRAM_T>(X, pitch, A, ldA, r0, nbuf_at(r0), r1, nt, 0, 0, pitch - 4, 1);
+  cq_fetch_factor<NBP, CQ_GRAM_T>(Lt, Ri, Lpk, (nt + 7) >> 3);
+  for (int rc = r0, nbuf = nbuf_at(r0), ntail = 0; rc < r1; rc += nbuf + ntail, nbuf = nbuf_at(rc)) {
+    ntail = split_at(rc) ? (r1 - rc - nbuf + 3) & ~3 : 0;
+    const int nact = nbuf + ntail;
+    if (rc > r0)
+      cq_issue_rows<CQ_GRAM_T>(X, pitch, A, ldA, rc, nbuf, r1, nt, 0, 0, pitch - 4, 1);
+    // the rows past the buffer into the scratch, zero-padded like the buffer (the solve then reads every row alike)
+    for (int e = threadIdx.x; e < ntail * (pitch - 4); e += CQ_GRAM_T) {
+      const int k = e / (pitch - 4), col = e - k * (pitch - 4), r = rc + nbuf + k;
+      tail[(size_t)k * pitch + col] = (r < r1 && col < nt) ? A[(size_t)r * ldA + col] : 0.0;
+    }
+    cpa_wait<0>();
+    __syncthreads();
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, g = lane >> 2, q = lane & 3, lr = 8 * wid + g;
+    // a row group is all in the buffer or all in the scratch
+    if (8 * wid < nbuf)
+      cq_solve_group<NH1, NH2>(X + (size_t)min(lr, nbuf - 1) * pitch, lr < nbuf, Lt, Ri, lane);
+    else if (8 * wid < nact)
+      cq_solve_group<NH1, NH2>(tail + (size_t)min(lr - nbuf, ntail - 1) * pitch, lr < nact, Lt, Ri, lane);
+    __syncthreads();
+    int ci, cj, offI, offJ;
+    bool diag;
+    const bool active = cq_tile_origin(0, wid, BW, 1, ci, cj, offI, offJ, diag);
+    double *part = Gpart + ((size_t)blockIdx.x * 16 + wid) * 1024 + g * 32 + 2 * q; // k_cq_gram's cs = 1 layout (one block)
+    if (active) {
+      double acc[4][4][2];
+#pragma unroll
+      for (int a = 0; a < 4; a++)
+#pragma unroll
+        for (int b = 0; b < 4; b++) {
+          const double2 v = rc > r0 ? *reinterpret_cast<const double2 *>(part + a * 256 + 8 * b) : make_double2(0.0, 0.0);
+          acc[a][b][0] = v.x;
+          acc[a][b][1] = v.y;
+        }
+      // the buffer's k-steps, then the scratch rows' where they are (a few k-steps: no second staging and barrier)
+#pragma unroll 1 // unrolled, the loads run ahead and the solve phase spills
+      for (int k = 0; k < nact; k += 4)
+        cq_gram_kstep(acc, k < nbuf ? X + (size_t)k * pitch : tail + (size_t)(k - nbuf) * pitch, pitch, offI, offJ, offI == offJ, g, q);
+#pragma unroll
+      for (int a = 0; a < 4; a++)
+#pragma unroll
+        for (int b = 0; b < 4; b++)
+          *reinterpret_cast<double2 *>(part + a * 256 + 8 * b) = make_double2(acc[a][b][0], acc[a][b][1]);
+    }
+    __syncthreads();
+  }
+}
+
+// Geometry of k_cq_solve_gram for slabs of slab_rows rows (a multiple of 4) and BW = ceil(nt / 32): buffer pitch, rows
+// the buffer takes per round, and rows per round solved into the scratch (ntail * pitch doubles per slab)
+struct CqSgShape {
+  int pitch, cb, ntail;
+};
+static CqSgShape cq_sg_shape(int nt, int BW, int slab_rows) {
+  const int NB = (nt + 7) / 8, NBP = NB <= 5 ? 5 : NB <= 10 ? 10 : NB <= 15 ? 15 : 20; // NH1 + NH2 of the instance cq_launch_solve_gram picks
+  CqSgShape s;
+  s.pitch = cq_sg_pitch(BW, NBP);
+  const int round = slab_rows < 8 * (CQ_GRAM_T / 32) ? slab_rows : 8 * (CQ_GRAM_T / 32);
+  const int fit = (int)((CQ_SG_SMEM - sizeof(double) * CQ_PK_DOUBLES) / (sizeof(double) * s.pitch)) & ~3;
+  s.cb = fit < round ? fit : round;
+  s.ntail = slab_rows > s.cb ? round - (s.cb & ~7) : 0; // the split last round: buffer rows end on a row-group boundary
+  return s;
+}
+// scratch doubles the launch below needs at Qtail
+static size_t cq_solve_gram_scratch(int nslab, int nt, int BW, int slab_rows) {
+  const CqSgShape s = cq_sg_shape(nt, BW, slab_rows);
+  return (size_t)nslab * s.ntail * s.pitch;
+}
+
+template <int NH1, int NH2>
+static void cq_launch_solve_gram_t(ovb_ctx *ctx, int nslab, const double *A, int ldA, int m, int nt, const double *Lpk, int slab_rows, int BW, double *Gpart,
+                                   double *Qtail) {
+  const CqSgShape s = cq_sg_shape(nt, BW, slab_rows);
+  const size_t smem = sizeof(double) * (CQ_PK_DOUBLES + (size_t)s.cb * s.pitch);
+  ovb_launch(ctx, k_cq_solve_gram<NH1, NH2>, dim3(nslab), dim3(CQ_GRAM_T), smem, A, ldA, m, nt, Lpk, slab_rows, s.cb, s.ntail, BW, Gpart, Qtail);
+}
+// slabs of slab_rows rows (a multiple of 4), BW = ceil(nt / 32): the Gram geometry of the narrow path; Qtail: scratch of
+// cq_solve_gram_scratch() doubles
+static void cq_launch_solve_gram(ovb_ctx *ctx, int nslab, const double *A, int ldA, int m, int nt, const double *Lpk, int slab_rows, int BW, double *Gpart,
+                                 double *Qtail) {
+  const int NB = (nt + 7) / 8;
+  if (NB <= 5)
+    cq_launch_solve_gram_t<5, 0>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail);
+  else if (NB <= 10)
+    cq_launch_solve_gram_t<10, 0>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail);
+  else if (NB <= 15)
+    cq_launch_solve_gram_t<10, 5>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail);
+  else
+    cq_launch_solve_gram_t<10, 10>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail);
 }
 
 // ------------------------------------------------------------------------------------------------------------ R = R2 R1
@@ -896,6 +1075,10 @@ static bool cq_attrs(ovb_ctx *ctx) {
     cudaFuncSetAttribute(k_cq_trsm<10, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
     cudaFuncSetAttribute(k_cq_trsm<10, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
     cudaFuncSetAttribute(k_cq_trsm<10, 10>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
+    cudaFuncSetAttribute(k_cq_solve_gram<5, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, CQ_SG_SMEM);
+    cudaFuncSetAttribute(k_cq_solve_gram<10, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, CQ_SG_SMEM);
+    cudaFuncSetAttribute(k_cq_solve_gram<10, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, CQ_SG_SMEM);
+    cudaFuncSetAttribute(k_cq_solve_gram<10, 10>, cudaFuncAttributeMaxDynamicSharedMemorySize, CQ_SG_SMEM);
     ctx->attr_done[4] = 1;
   }
   return true;
@@ -1083,8 +1266,10 @@ static int cq_compress_wide(ovb_ctx *ctx, double *A, int m, int n, int ldA, doub
   return launches + 1;
 }
 
-// [R | z] <- shifted CholeskyQR2 of A [m x (n+1)] (A is overwritten by Q1). Returns the number of kernels launched, or -1
-// when the system is too wide for this path (the caller falls back to the Householder TSQR).
+// [R | z] <- shifted CholeskyQR2 of A [m x (n+1)]: pass 1 k_cq_gram -> k_cq_reduce -> k_cq_chol_gram, pass 2
+// k_cq_solve_gram (Q1 = A R1^-1 and its Gram partials in one kernel) -> k_cq_reduce -> k_cq_chol_gram, then k_cq_trmm.
+// A is left unchanged here (the wide path overwrites it with Q1). Returns the number of kernels launched, or -1 when the
+// system is too wide for this path (the caller falls back to the Householder TSQR).
 int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR) {
   const int nt = n + 1;
   if ((ldA & 1) || m < 1)
@@ -1104,7 +1289,8 @@ int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, doub
   // clusters of CQ_GRAM_CS slabs pre-reduce their partial tiles in distributed shared memory (empty slabs pad the grid)
   const int cs = (ctx->gram_cluster && nslab >= 2 * CQ_GRAM_CS) ? CQ_GRAM_CS : 1;
   const int nslab_pad = (nslab + cs - 1) / cs * cs, npart = nslab_pad / cs;
-  const size_t need_part = (size_t)nslab_pad * nblk * 16 * 1024;
+  const size_t part_doubles = (size_t)nslab_pad * nblk * 16 * 1024;
+  const size_t need_part = part_doubles + cq_solve_gram_scratch(nslab, nt, BW, slab_rows); // partials | pass-2 row scratch
   const int ldW = CQ_MAXN + 8;
   if (!cq_ensure_G(ctx))
     return -1;
@@ -1121,20 +1307,16 @@ int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, doub
   size_t gram_smem = sizeof(double) * 2 * CQ_KB * (size_t)(BW * 32 + 4);
   if (cs > 1 && gram_smem < sizeof(double) * 16 * 1024)
     gram_smem = sizeof(double) * 16 * 1024; // staging of the 16 warp tiles for the cluster reduction
-  const int ngroups = (m + 7) / 8;
-  int trsm_ctas = (ngroups + CQ_TRSM_T / 32 - 1) / (CQ_TRSM_T / 32);
-  if (trsm_ctas > ctx->sm_count)
-    trsm_ctas = ctx->sm_count;
-  for (int pass = 0; pass < 2; pass++) {
-    cq_launch_gram(ctx, nblk, nslab_pad, gram_smem, (const double *)A, ldA, m, nt, slab_rows, BW, nblk_side, ctx->d_Gpart, cs);
-    ovb_launch(ctx, k_cq_reduce, dim3(CQ_RED_GX, nblk), dim3(CQ_RED_T), (size_t)0, (const double *)ctx->d_Gpart, npart, nblk, BW, nblk_side, nt, G, ldW, 1);
-    ovb_launch(ctx, k_cq_chol_gram, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), (const double *)G, ldW, nt, pass == 0 ? 1e-11 : 1e-13,
-               pass == 0 ? L1 : L2, 1);
-    if (pass == 0)
-      cq_launch_trsm(ctx, trsm_ctas, A, ldA, m, nt, (const double *)L1);
-  }
+  // pass 1: G1 = A'A -> R1
+  cq_launch_gram(ctx, nblk, nslab_pad, gram_smem, (const double *)A, ldA, m, nt, slab_rows, BW, nblk_side, ctx->d_Gpart, cs);
+  ovb_launch(ctx, k_cq_reduce, dim3(CQ_RED_GX, nblk), dim3(CQ_RED_T), (size_t)0, (const double *)ctx->d_Gpart, npart, nblk, BW, nblk_side, nt, G, ldW, 1);
+  ovb_launch(ctx, k_cq_chol_gram, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), (const double *)G, ldW, nt, 1e-11, L1, 1);
+  // pass 2: G2 = Q1'Q1 (one partial per slab, no cluster) -> R2
+  cq_launch_solve_gram(ctx, nslab, (const double *)A, ldA, m, nt, (const double *)L1, slab_rows, BW, ctx->d_Gpart, ctx->d_Gpart + part_doubles);
+  ovb_launch(ctx, k_cq_reduce, dim3(CQ_RED_GX, nblk), dim3(CQ_RED_T), (size_t)0, (const double *)ctx->d_Gpart, nslab, nblk, BW, nblk_side, nt, G, ldW, 1);
+  ovb_launch(ctx, k_cq_chol_gram, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), (const double *)G, ldW, nt, 1e-13, L2, 1);
   const int nT16 = (nt + 15) / 16;
   ovb_launch(ctx, k_cq_trmm, dim3(nT16, nT16), dim3(256), (size_t)0, (const double *)L2, (const double *)L1, nt, Rout, ldR);
-  ctx->n_launch += 8;
-  return 8;
+  ctx->n_launch += 7;
+  return 7;
 }

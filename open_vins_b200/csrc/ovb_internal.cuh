@@ -195,8 +195,8 @@ void launch_tsqr(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, i
 // gather columns of Rin in the order info->col_canon (n_used of them) into Hs scratch and re-triangularise into Rout
 // [R | z] <- chol([H r]'[H r]) (k_gram.cu); returns the number of kernels launched or -1
 int launch_compress_gram(ovb_ctx *ctx, const double *A, int m, int n, int ldA, double *Rout, int ldR);
-// [R | z] <- shifted CholeskyQR2 of A (k_cholqr.cu; A is overwritten); returns kernels launched, or -1 when n+1 exceeds
-// what the single-CTA Cholesky takes (callers then use launch_tsqr)
+// [R | z] <- shifted CholeskyQR2 of A (k_cholqr.cu; A is kept up to CQ_MAXN columns, overwritten by the wider blocked
+// path); returns kernels launched, or -1 when the system is too wide for it (callers then use launch_tsqr)
 int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR);
 // EKF Cholesky on the DMMA kernel of k_cholqr.cu; false when r does not fit (caller uses k_ekf_chol)
 bool launch_chol_ekf_dmma(ovb_ctx *ctx, double *S, int ldS, int r, const double *res, double *w, double *invdiag, double **Lpk_out);
