@@ -258,11 +258,22 @@ typedef struct {
 /* UpdaterSLAM::update steps 4-5 (update/UpdaterSLAM.cpp:310-470): per-feature Jacobians with the landmark's own 3
  * columns appended (H_xf = [H_x, H_f], no nullspace projection), chi² gate on the marginal of (H_x variables + landmark),
  * stacking and ONE EKF update of the whole batch. The reference does not compress this system; the engine whitens the
- * rows by 1/sigma and compresses when rows > columns, which leaves the posterior unchanged. At most OVB_MAX_VARS (64)
- * state variables (clones + calibration blocks + landmarks) per call: batch like max_slam_in_update does.
+ * rows by 1/sigma and compresses when rows > columns, which leaves the posterior unchanged.
+ * Batch size: a new context takes at most OVB_MAX_VARS state variables (clones + calibration blocks + landmarks) per call
+ * and returns OVB_ERR_CAPACITY beyond. After ovb_set_slam_unbounded(ctx, 1) any batch that fits the context's max_feats,
+ * max_meas and max_state is one call, whatever its number of landmarks (max_slam_in_update as in the reference, e.g. 100
+ * for SURVEY.md config 4). Every gate sees the prior P.
+ * A batch wider than 512 columns (frame columns + landmark columns) is cut into column groups, contiguous feature ranges
+ * whose frame plus landmark columns fit 512; the groups are applied as sequential EKF updates at the same linearization
+ * point, each group's compressed residual corrected by the state change of the groups before it, which equals the single
+ * update to rounding. Such a batch is updated in its groups' canonical column order whatever opts->col_order says (the
+ * order only changes rounding), and on any EKF failure (not SPD, negative diagonal, non-finite) P keeps its prior and dx
+ * is zero.
  * out->status: OVB_FEAT_OK or OVB_FEAT_CHI2; out->chi2 filled; p_FinA/p_FinG/anchor_* are not written. */
 ovb_status ovb_slam_update(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_batch *feats, const ovb_landmarks *landmarks,
                            const ovb_opts *opts, ovb_feat_out *out, double *dx, ovb_stats *stats);
+/* enabled = 1: ovb_slam_update accepts batches of more than OVB_MAX_VARS state variables (see above); 0: the default. */
+ovb_status ovb_set_slam_unbounded(ovb_ctx *ctx, int enabled);
 
 /* UpdaterSLAM::delayed_init (update/UpdaterSLAM.cpp:61-251) in ONE call: triangulate + Gauss-Newton every new track (:118-142),
  * then, one feature after the other like the reference (each StateHelper::initialize mutates the covariance AND the state

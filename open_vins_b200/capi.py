@@ -289,6 +289,7 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.ovb_set_profile.argtypes = [vp, C.c_int]
     lib.ovb_profile_read.argtypes = [vp, C.c_char_p, C.c_int, c_float_p, C.c_int, c_int_p]
     lib.ovb_set_replay.argtypes = [vp, C.c_int]
+    lib.ovb_set_slam_unbounded.argtypes = [vp, C.c_int]
     lib.ovb_msckf_replay.argtypes = [vp, C.c_int, C.c_int, c_float_p, C.POINTER(C.c_float * 5)]
     if path is None:
         _LIB = lib
@@ -298,7 +299,7 @@ def load_library(path: str | None = None) -> C.CDLL:
 EXPORTED_SYMBOLS = [
     "ovb_create", "ovb_destroy", "ovb_last_error", "ovb_abi_version", "ovb_opts_default", "ovb_cov_set", "ovb_cov_get",
     "ovb_cov_dim", "ovb_cov_get_marginal", "ovb_cov_clone", "ovb_cov_marginalize", "ovb_cov_propagate", "ovb_cov_initialize",
-    "ovb_msckf_update", "ovb_slam_update", "ovb_slam_delayed_init", "ovb_slam_anchor_change", "ovb_ekf_update", "ovb_triangulate", "ovb_feature_jacobians", "ovb_compress", "ovb_compress_gram", "ovb_compress_cholqr2",
+    "ovb_msckf_update", "ovb_slam_update", "ovb_set_slam_unbounded", "ovb_slam_delayed_init", "ovb_slam_anchor_change", "ovb_ekf_update", "ovb_triangulate", "ovb_feature_jacobians", "ovb_compress", "ovb_compress_gram", "ovb_compress_cholqr2",
     "ovb_chi2_quantile95", "ovb_last_stage_ms", "ovb_set_replay", "ovb_msckf_replay", "ovb_last_counters", "ovb_last_host_us", "ovb_set_profile", "ovb_profile_read",
     "ovb_set_stream", "ovb_msckf_shard_compress", "ovb_msckf_shard_compress_range", "ovb_shard_partition", "ovb_msckf_shard_finish",
 ]
@@ -447,6 +448,10 @@ class Engine:
                                       _ptr(dx, c_double_p), C.byref(stats))
         self._check(st, allow=(OVB_ERR_NEG_DIAG,))
         return st, out, dx, stats
+
+    def set_slam_unbounded(self, enabled=True):
+        """slam_update accepts batches of more than OVB_MAX_VARS state variables (off by default)"""
+        self._check(self.lib.ovb_set_slam_unbounded(self.h, int(enabled)))
 
     def slam_delayed_init(self, frame: FrameArrays, feats: FeatArrays, opts: ovb_opts, on_init=None, sigma_pix=None, chi2_multipler=None):
         """UpdaterSLAM::delayed_init in one call. on_init(feat_index, lm_off, dx_new, dx) must apply dx to the caller's state and

@@ -757,6 +757,126 @@ void launch_column_map(ovb_ctx *ctx, int n_feats, BlobView bv, int rows_drop) {
   k_column_map<<<1, 256, 0, ctx->stream>>>(ctx->d_frame, ctx->d_opts, ctx->d_feat, n_feats, ovb_feat_order_ptr(ctx), ctx->d_info, rows_drop);
 }
 
+// SLAM update: the variables are the frame's slots plus one landmark per feature. A feature's landmark is the last entry of
+// its Hxf_order and never seen before it (UpdaterSLAM.cpp:385-387), so its first-seen key is (f, number of frame entries
+// of the feature). The counts cover the whole batch; full_map (a batch of one column group) also writes the column map of
+// the group's layout exactly as k_column_map does for slots (unused variables last, in canonical order).
+#define CM_MAX_ENT (OVB_MAX_VARS + OVB_MAX_COLS)
+__global__ void k_column_map_slam(const DevFrame *__restrict__ fr, const DevOpts *__restrict__ dop, const DevFeat *__restrict__ feats, int n_feats,
+                                  const unsigned char *__restrict__ feat_order, DevUpdateInfo *__restrict__ info, int rows_drop, int lmw,
+                                  int full_map) {
+  __shared__ unsigned int key[OVB_MAX_VARS];
+  __shared__ unsigned int ekey[CM_MAX_ENT];
+  __shared__ int order[CM_MAX_ENT];
+  __shared__ int n_used_feats, rows_stacked;
+  const int tid = threadIdx.x;
+  if (tid < OVB_MAX_VARS)
+    key[tid] = 0xffffffffu;
+  if (tid == 0) {
+    n_used_feats = 0;
+    rows_stacked = 0;
+  }
+  __syncthreads();
+  for (int f = tid; f < n_feats; f += blockDim.x) {
+    if (feats[f].status != OVB_FEAT_OK)
+      continue;
+    atomicAdd(&n_used_feats, 1);
+    atomicAdd(&rows_stacked, 2 * (feats[f].m1 - feats[f].m0) - rows_drop);
+    const unsigned char *ord = feat_order + (size_t)f * (OVB_MAX_VARS + 1);
+    int no = ord[0];
+    for (int q = 0; q < no; q++)
+      atomicMin(&key[ord[1 + q]], ((unsigned int)f << 7) | (unsigned int)q);
+  }
+  __syncthreads();
+  const int n_slots = fr->n_slots;
+  if (!full_map) {
+    if (tid == 0) {
+      int used_cols = 0, n_order = 0;
+      for (int s = 0; s < n_slots; s++)
+        if (key[s] != 0xffffffffu) {
+          used_cols += fr->slot_size[s];
+          n_order++;
+        }
+      info->n_order = n_order + n_used_feats;
+      info->n_used = used_cols + n_used_feats * lmw;
+      info->n_feats_used = n_used_feats;
+      info->rows_stacked = rows_stacked;
+      info->neg_diag_index = -1;
+      info->not_spd = 0;
+      info->nonfinite = 0;
+    }
+    return;
+  }
+  const DevGroup *G = fr->groups;
+  const int n_ent = G->n_ent;
+  for (int i = tid; i < n_ent; i += blockDim.x) {
+    const int e = G->ent[i];
+    if (e >= 0) {
+      ekey[i] = key[e];
+    } else {
+      const int f = -1 - e;
+      ekey[i] = feats[f].status == OVB_FEAT_OK ? (((unsigned int)f << 7) | (unsigned int)feat_order[(size_t)f * (OVB_MAX_VARS + 1)]) : 0xffffffffu;
+    }
+  }
+  __syncthreads();
+  const bool first_seen = (dop->o.col_order == OVB_COLS_REFERENCE_FIRST_SEEN);
+  for (int i = tid; i < n_ent; i += blockDim.x) {
+    // rank among used variables: first-seen order = ascending key; canonical = ascending entry (covariance offset)
+    int rank = 0, nused = 0, r2 = 0;
+    for (int t = 0; t < n_ent; t++) {
+      const bool used = ekey[t] != 0xffffffffu;
+      nused += used ? 1 : 0;
+      r2 += (!used && t < i) ? 1 : 0;
+      if (used && (first_seen ? (ekey[t] < ekey[i]) : (t < i)))
+        rank++;
+    }
+    if (!first_seen)
+      order[i] = i; // canonical layout: stacked column q IS canonical column q (unused variables stay as zero columns)
+    else if (ekey[i] != 0xffffffffu)
+      order[rank] = i;
+    else
+      order[nused + r2] = i; // unused variables go last, in canonical order (their columns are all zero)
+  }
+  __syncthreads();
+  if (tid == 0) {
+    // canonical column of every entry, then the stacked map in the chosen order
+    int c = 0;
+    for (int i = 0; i < n_ent; i++) {
+      const int e = G->ent[i];
+      ekey[i] = (unsigned int)c; // ekey is free now: canonical start column
+      c += e >= 0 ? fr->slot_size[e] : lmw;
+    }
+    int col = 0, used_cols = 0, n_order = 0;
+    for (int q = 0; q < n_ent; q++) {
+      const int i = order[q], e = G->ent[i];
+      const int off = e >= 0 ? fr->slot_off[e] : feats[-1 - e].lm_off;
+      const int sz = e >= 0 ? fr->slot_size[e] : lmw;
+      const bool used = e >= 0 ? key[e] != 0xffffffffu : feats[-1 - e].status == OVB_FEAT_OK;
+      for (int k = 0; k < sz; k++) {
+        info->col_state[col] = off + k;
+        info->col_canon[col] = (int)ekey[i] + k;
+        col++;
+      }
+      if (used) {
+        used_cols += sz;
+        n_order++;
+      }
+    }
+    info->n_order = n_order;
+    info->n_used = used_cols;
+    info->n_feats_used = n_used_feats;
+    info->rows_stacked = rows_stacked;
+    info->neg_diag_index = -1;
+    info->not_spd = 0;
+    info->nonfinite = 0;
+  }
+}
+
+void launch_column_map_slam(ovb_ctx *ctx, int n_feats, int rows_drop, int lmw, bool full_map) {
+  k_column_map_slam<<<1, 256, 0, ctx->stream>>>(ctx->d_frame, ctx->d_opts, ctx->d_feat, n_feats, ovb_feat_order_ptr(ctx), ctx->d_info, rows_drop,
+                                                lmw, full_map ? 1 : 0);
+}
+
 // B[i][q] = Rin[i][col_canon[q]] for q < n_all, B[i][n_all] = Rin[i][n_all] (residual)
 __global__ void k_gather_cols(const double *__restrict__ Rin, int ldRin, int n_all, const DevUpdateInfo *__restrict__ info, double *__restrict__ B,
                               int ldB) {

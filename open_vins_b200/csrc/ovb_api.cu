@@ -188,11 +188,11 @@ void ovb_destroy(ovb_ctx *ctx) {
     cudaStreamSynchronize(ctx->stream);
   void *dev[] = {ctx->P[0],   ctx->P[1], ctx->d_arena, ctx->d_cc, ctx->d_feat_order, ctx->d_info, ctx->d_chi2_table, ctx->d_Hs, ctx->d_W[0],
                  ctx->d_W[1], ctx->d_R,  ctx->d_R2,    ctx->d_M,  ctx->d_S,          ctx->d_Y,    ctx->d_w,          ctx->d_scratch,
-                 ctx->d_long, ctx->d_dump, ctx->P_snap, ctx->d_flush, ctx->d_Gpart, ctx->d_G, ctx->d_cqw};
+                 ctx->d_long, ctx->d_dump, ctx->P_snap, ctx->d_flush, ctx->d_Gpart, ctx->d_G, ctx->d_cqw, ctx->d_grp, ctx->d_grp_acc};
   for (void *p : dev)
     if (p)
       cudaFree(p);
-  void *host[] = {ctx->h_arena, ctx->h_info, ctx->h_stage};
+  void *host[] = {ctx->h_arena, ctx->h_info, ctx->h_stage, ctx->h_grp};
   for (void *p : host)
     if (p)
       cudaFreeHost(p);
@@ -349,11 +349,97 @@ ovb_status ovb_cov_propagate(ovb_ctx *ctx, int new_off, int p, const int *old_of
 // ------------------------------------------------------------------------------------------------ marshalling
 struct Packed {
   int n_feats, n_meas, m_total, ldH, n_all;
+  int n_groups; // SLAM: column groups (ctx->h_grp / d_grp); n_all is then the widest group's column count
   BlobView bv;
 };
 
-// lm != nullptr: SLAM batch — every feature brings its landmark (a 3-wide state variable that becomes one more slot),
-// rows are NOT nullspace-projected (2M per feature instead of 2M-3), values/anchors come from the landmark.
+// group tables for n groups; several groups also need the prior's snapshot and the correction accumulator
+static ovb_status ensure_groups(ovb_ctx *ctx, int n) {
+  if (n > 1) {
+    if (!ctx->P_snap)
+      OVB_CUDA_CHECK(ctx, cudaMalloc(&ctx->P_snap, sizeof(double) * (size_t)ctx->ldP * ctx->ldP));
+    if (!ctx->d_grp_acc)
+      OVB_CUDA_CHECK(ctx, cudaMalloc(&ctx->d_grp_acc, sizeof(double) * ((size_t)ctx->cfg.max_state + 4)));
+  }
+  if (n <= ctx->grp_cap)
+    return OVB_OK;
+  if (ctx->d_grp)
+    cudaFree(ctx->d_grp);
+  if (ctx->h_grp)
+    cudaFreeHost(ctx->h_grp);
+  ctx->d_grp = nullptr;
+  ctx->h_grp = nullptr;
+  ctx->grp_cap = 0;
+  const int cap = std::max(n, 4);
+  OVB_CUDA_CHECK(ctx, cudaMalloc(&ctx->d_grp, sizeof(DevGroup) * (size_t)cap));
+  OVB_CUDA_CHECK(ctx, cudaMallocHost(&ctx->h_grp, sizeof(DevGroup) * (size_t)cap));
+  ctx->grp_cap = cap;
+  return OVB_OK;
+}
+
+// Column groups of a SLAM batch (h_feat / h_frame packed): features in input order, as many landmarks per group as fit
+// next to the frame's columns in OVB_MAX_COLS. A group's layout is its canonical layout, the frame slots and its landmarks
+// in ascending covariance offset (a batch of one group: the batch's canonical layout). Rows are stacked in input order, so
+// a group's rows are contiguous.
+static ovb_status build_groups(ovb_ctx *ctx, int F, int rows_total, int lmw, Packed *pk) {
+  const DevFrame *hf = ctx->h_frame;
+  const int per = (OVB_MAX_COLS - hf->n_all) / lmw; // hf->n_all <= 6 OVB_MAX_CLONES + 14 OVB_MAX_CAMS < OVB_MAX_COLS
+  const int G = (F + per - 1) / per;
+  if (per < 1 || G > 0xffff) {
+    snprintf(ctx->err, sizeof(ctx->err), "SLAM batch of %d landmarks: %d column groups", F, G);
+    return OVB_ERR_CAPACITY;
+  }
+  ovb_status st = ensure_groups(ctx, G);
+  if (st != OVB_OK)
+    return st;
+  int widest = 0;
+  std::vector<std::pair<int, int>> lms; // (offset, feature)
+  for (int g = 0; g < G; g++) {
+    DevGroup &gr = ctx->h_grp[g];
+    gr.f0 = g * per;
+    gr.f1 = std::min(F, gr.f0 + per);
+    gr.row0 = ctx->h_feat[gr.f0].row0;
+    gr.rows = (gr.f1 < F ? ctx->h_feat[gr.f1].row0 : rows_total) - gr.row0;
+    lms.clear();
+    for (int f = gr.f0; f < gr.f1; f++)
+      lms.push_back({ctx->h_feat[f].lm_off, f});
+    std::sort(lms.begin(), lms.end());
+    int col = 0, n_ent = 0;
+    size_t l = 0;
+    for (int s = 0; s < hf->n_slots || l < lms.size();) {
+      if (l < lms.size() && (s == hf->n_slots || lms[l].first < hf->slot_off[s])) {
+        const int f = lms[l++].second;
+        gr.ent[n_ent++] = -1 - f;
+        ctx->h_feat[f].lm_col = (unsigned short)col;
+        ctx->h_feat[f].grp = (unsigned short)g;
+        for (int k = 0; k < lmw; k++, col++) {
+          gr.col_frame[col] = -1;
+          gr.col_state[col] = ctx->h_feat[f].lm_off + k;
+        }
+      } else {
+        gr.ent[n_ent++] = s;
+        for (int k = 0; k < hf->slot_size[s]; k++, col++) {
+          gr.col_frame[col] = (short)(hf->slot_col[s] + k);
+          gr.col_state[col] = hf->slot_off[s] + k;
+        }
+        s++;
+      }
+    }
+    gr.n_cols = col;
+    gr.n_ent = n_ent;
+    widest = std::max(widest, col);
+  }
+  if (widest + 1 > std::min(OVB_MAX_COLS, ctx->cfg.max_state) + 8)
+    return OVB_ERR_CAPACITY;
+  pk->n_groups = G;
+  pk->n_all = widest;
+  return OVB_OK;
+}
+
+// lm != nullptr: SLAM batch — every feature brings its landmark (a 3-wide state variable, or 1-wide for
+// ANCHORED_INVERSE_DEPTH_SINGLE), rows are NOT nullspace-projected (2M per feature instead of 2M-3), values/anchors come
+// from the landmark. The landmarks are not frame slots: the batch is cut into column groups (DevGroup), contiguous feature
+// ranges whose frame columns plus landmark columns fit OVB_MAX_COLS.
 // per_feature: the call will launch the per-feature kernel (everything but ovb_triangulate), so its scratch is reserved.
 static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_batch *fb, const ovb_opts *op, const ovb_feat_out *given,
                               Packed *pk, const ovb_landmarks *lm = nullptr, bool per_feature = true) {
@@ -388,11 +474,8 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
     int off, size, kind, idx;
   }; // kind 0 clone, 1 ext, 2 intr, 3 landmark
   std::vector<SlotRec> slots;
-  std::vector<int> lm_slot_of((size_t)(lm ? fb->n_feats : 0), -1);
   const bool lm_single = lm && op->feat_rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE; // 1-wide landmark (inverse depth only)
-  if (lm)
-    for (int f = 0; f < fb->n_feats; f++)
-      slots.push_back({lm->lm_off[f], lm_single ? 1 : 3, 3, f});
+  const int lmw = lm_single ? 1 : 3;
   for (int k = 0; k < fr->n_cams; k++) {
     hf->cam_ext_slot[k] = hf->cam_intr_slot[k] = -1;
     if (op->do_calib_camera_pose) {
@@ -413,9 +496,14 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
   for (int c = 0; c < fr->n_clones; c++)
     slots.push_back({fr->clone_off[c], 6, 0, c});
   std::sort(slots.begin(), slots.end(), [](const SlotRec &a, const SlotRec &b) { return a.off < b.off; });
-  if ((int)slots.size() > OVB_MAX_VARS) {
-    snprintf(ctx->err, sizeof(ctx->err), "%d state variables in one update (clones + calibration + landmarks), max %d: split the batch",
-             (int)slots.size(), OVB_MAX_VARS);
+  if ((int)slots.size() > OVB_MAX_VARS) { // clones + calibration: OVB_MAX_CLONES + 2 OVB_MAX_CAMS at most
+    snprintf(ctx->err, sizeof(ctx->err), "%d frame variables (clones + calibration), max %d", (int)slots.size(), OVB_MAX_VARS);
+    return OVB_ERR_CAPACITY;
+  }
+  if (lm && !ctx->slam_unbounded && (int)slots.size() + fb->n_feats > OVB_MAX_VARS) {
+    snprintf(ctx->err, sizeof(ctx->err),
+             "%d state variables in one update (clones + calibration + landmarks), max %d: split the batch or ovb_set_slam_unbounded",
+             (int)slots.size() + fb->n_feats, OVB_MAX_VARS);
     return OVB_ERR_CAPACITY;
   }
   int col = 0;
@@ -436,15 +524,32 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
       hf->clone_slot[slots[s].idx] = (int)s;
     else if (slots[s].kind == 1)
       hf->cam_ext_slot[slots[s].idx] = (int)s;
-    else if (slots[s].kind == 2)
-      hf->cam_intr_slot[slots[s].idx] = (int)s;
     else
-      lm_slot_of[(size_t)slots[s].idx] = (int)s;
+      hf->cam_intr_slot[slots[s].idx] = (int)s;
   }
   hf->n_slots = (int)slots.size();
   hf->n_all = col;
+  hf->groups = nullptr;
   if (col > OVB_MAX_COLS || col + 1 > std::min(OVB_MAX_COLS, ctx->cfg.max_state) + 8)
     return OVB_ERR_CAPACITY;
+  if (lm) { // landmarks: inside the covariance, overlapping neither a frame variable nor each other
+    std::vector<std::pair<int, int>> all; // (offset, size)
+    for (const SlotRec &r : slots)
+      all.push_back({r.off, r.size});
+    for (int f = 0; f < fb->n_feats; f++)
+      all.push_back({lm->lm_off[f], lmw});
+    std::sort(all.begin(), all.end());
+    for (size_t s = 0; s < all.size(); s++) {
+      if (all[s].first < 0 || all[s].first + all[s].second > ctx->N) {
+        snprintf(ctx->err, sizeof(ctx->err), "variable offset %d(+%d) outside the covariance (N=%d)", all[s].first, all[s].second, ctx->N);
+        return OVB_ERR_ARG;
+      }
+      if (s > 0 && all[s].first < all[s - 1].first + all[s - 1].second) {
+        snprintf(ctx->err, sizeof(ctx->err), "overlapping state variables at offset %d", all[s].first);
+        return OVB_ERR_ARG;
+      }
+    }
+  }
   // ---- options
   DevOpts *ho = ctx->h_opts;
   ho->o = *op;
@@ -538,11 +643,12 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
       d.p_FinA[k] = d.p_FinG[k] = NAN;
     d.sigma_sq = std::pow(op->sigma_pix, 2);
     d.chi2_mult = op->chi2_multipler;
-    d.lm_slot = -1;
+    d.lm_off = -1;
+    d.lm_col = d.grp = 0;
     for (int k = 0; k < 3; k++)
       d.p_FinG_fej[k] = NAN;
     if (lm) {
-      d.lm_slot = lm_slot_of[(size_t)f];
+      d.lm_off = lm->lm_off[f];
       d.status = Mf >= (lm_single ? 2 : 1) ? OVB_FEAT_OK : OVB_FEAT_FEW_MEAS; // UpdaterSLAM.cpp:278-290
       const bool rel = op->feat_rep >= OVB_REP_ANCHORED_3D;
       d.anchor_cam = rel && lm->anchor_cam ? lm->anchor_cam[f] : -1;
@@ -585,8 +691,15 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
   pk->n_meas = M;
   pk->m_total = row;
   pk->n_all = col;
-  pk->ldH = (int)align_up((size_t)col + 1, 4);
-  if ((size_t)std::max(row, col) * pk->ldH > ctx->Hs_cap || row > ctx->max_rows) {
+  pk->n_groups = 0;
+  if (lm) {
+    ovb_status gs = build_groups(ctx, F, row, lmw, pk);
+    if (gs != OVB_OK)
+      return gs;
+    hf->groups = ctx->d_grp;
+  }
+  pk->ldH = (int)align_up((size_t)pk->n_all + 1, 4);
+  if ((size_t)std::max(row, pk->n_all) * pk->ldH > ctx->Hs_cap || row > ctx->max_rows) {
     snprintf(ctx->err, sizeof(ctx->err), "stacked system %d x %d exceeds the reserved staging matrix", row, pk->ldH);
     return OVB_ERR_CAPACITY;
   }
@@ -603,6 +716,10 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
   size_t used = ctx->off_blob + o_keys + nkeys;
   ctx->last_h2d_bytes = used;
   cudaError_t e = cudaMemcpyAsync(ctx->d_arena, ctx->h_arena, used, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess && pk->n_groups > 0) {
+    e = cudaMemcpyAsync(ctx->d_grp, ctx->h_grp, sizeof(DevGroup) * (size_t)pk->n_groups, cudaMemcpyHostToDevice, ctx->stream);
+    ctx->last_h2d_bytes += sizeof(DevGroup) * (size_t)pk->n_groups;
+  }
   if (e != cudaSuccess) {
     snprintf(ctx->err, sizeof(ctx->err), "H2D arena copy: %s", cudaGetErrorString(e));
     return OVB_ERR_CUDA;
@@ -837,6 +954,54 @@ __global__ void k_fill_zero_dx(double *dx, int N) {
     dx[i] = 0.0;
 }
 
+// ---- SLAM batches of several column groups: sequential EKF updates at one linearization point. With the rows whitened
+// (R = I), group g's compressed system [R_g | z_g] is applied to the mean already corrected by the groups before it,
+// z_g <- z_g - R_g dx_acc[cols_g]; the result equals the joint update (tests/test_slam_batches_cpu.py).
+// Copies the group's column map into info (the EKF reads it there) and stages the corrected residual in w.
+__global__ void k_group_take_z(const double *__restrict__ R, int ldR, int rows, int n, const int *__restrict__ col_state,
+                               const double *__restrict__ dx_acc, double *__restrict__ w, DevUpdateInfo *__restrict__ info) {
+  OVB_PDL_ENTER();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n)
+    info->col_state[i] = col_state[i];
+  if (i < rows) {
+    const double *Ri = R + (size_t)i * ldR;
+    double z = Ri[n];
+    for (int j = 0; j < n; j++)
+      z -= Ri[j] * dx_acc[col_state[j]];
+    w[i] = z;
+  }
+}
+// dx_acc += dx of the group; the group's failure flags are kept (the next group's EKF resets them in info)
+__global__ void k_group_accumulate(const double *__restrict__ dx, double *__restrict__ dx_acc, int N, const DevUpdateInfo *__restrict__ info,
+                                   int *__restrict__ flags) {
+  OVB_PDL_ENTER();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N)
+    dx_acc[i] += dx[i];
+  if (i == 0) {
+    if (info->not_spd)
+      flags[0] = 1;
+    if (info->nonfinite)
+      flags[1] = 1;
+  }
+}
+// after the last group: dx = dx_acc, or on any failure (not SPD, non-finite, negative diagonal) dx = 0 and P = the prior
+__global__ void k_group_finish(double *__restrict__ P, int ldP, int N, const double *__restrict__ P_prior, const double *__restrict__ dx_acc,
+                               double *__restrict__ dx, DevUpdateInfo *__restrict__ info, const int *__restrict__ flags) {
+  OVB_PDL_ENTER();
+  const bool failed = flags[0] || flags[1] || info->neg_diag_index != 0x7fffffff;
+  const int j = blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y * blockDim.y + threadIdx.y;
+  if (i == 0 && j < N)
+    dx[j] = failed ? 0.0 : dx_acc[j];
+  if (i == 0 && j == 0) {
+    info->not_spd = flags[0];
+    info->nonfinite = flags[1];
+  }
+  if (failed && i < N && j < N)
+    P[(size_t)i * ldP + j] = P_prior[(size_t)i * ldP + j];
+}
+
 // measurement_compress_inplace in the requested mode; returns the number of rows of [R | z] handed to the EKF update.
 // The Cholesky-based modes always produce n rows; the Householder path leaves min(m, n).
 static int compress_system(ovb_ctx *ctx, int mode, double *A, int m, int n, int ldA, double *Rout, int ldR) {
@@ -851,9 +1016,12 @@ static int compress_system(ovb_ctx *ctx, int mode, double *A, int m, int n, int 
 // The device pipeline of one update on inputs already in the arena: steps 2-6 of UpdaterMSCKF::update.
 // ev (optional): ev[1] after triangulation, ev[2] after the per-feature systems, ev[3] after the column map, ev[4] after
 // compression, ev[5] after the EKF update. Returns the row count handed to the EKF update.
-// slam: UpdaterSLAM::update — landmarks come from the state (no triangulation), rows are kept unprojected and whitened.
+// slam: UpdaterSLAM::update — landmarks come from the state (no triangulation), rows are kept unprojected and whitened;
+// n_groups column groups (ctx->h_grp). Several groups: every gate sees the prior P (the per-feature kernel runs once over
+// the batch), then each group is compressed and applied in turn (ev[4] then marks the start of that loop).
+static int enqueue_slam_groups(ovb_ctx *ctx, int n_groups, int ldH);
 static int enqueue_update(ovb_ctx *ctx, int F, BlobView bv, int ldH, int m_total, int n_all, int col_order, cudaEvent_t *ev,
-                          bool slam = false) {
+                          bool slam = false, int n_groups = 1) {
   const int N = ctx->N;
   ctx->n_launch = 0;
   ctx->n_launch_tsqr_level = 0;
@@ -876,12 +1044,26 @@ static int enqueue_update(ovb_ctx *ctx, int F, BlobView bv, int ldH, int m_total
     cudaStreamWaitEvent(ctx->side_stream, ctx->ev_fork, 0);
     cudaStream_t main_stream = ctx->stream;
     ctx->stream = ctx->side_stream;
-    launch_column_map(ctx, F, bv, slam ? (ctx->h_opts->o.feat_rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE ? 2 : 0) : 3);
+    if (slam) {
+      const bool single = ctx->h_opts->o.feat_rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE;
+      launch_column_map_slam(ctx, F, single ? 2 : 0, single ? 1 : 3, n_groups == 1);
+    } else {
+      launch_column_map(ctx, F, bv, 3);
+    }
     ctx->stream = main_stream;
     cudaEventRecord(ctx->ev_join, ctx->side_stream);
   }
   if (ev)
     cudaEventRecord(ev[3], ctx->stream);
+  if (slam && n_groups > 1) {
+    cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0);
+    if (ev)
+      cudaEventRecord(ev[4], ctx->stream);
+    const int r = enqueue_slam_groups(ctx, n_groups, ldH);
+    if (ev)
+      cudaEventRecord(ev[5], ctx->stream);
+    return r;
+  }
   const int ldR = ldH;
   const double *Rfinal = ctx->d_R;
   int r = 0;
@@ -908,6 +1090,38 @@ static int enqueue_update(ovb_ctx *ctx, int F, BlobView bv, int ldH, int m_total
   if (ev)
     cudaEventRecord(ev[5], ctx->stream);
   return r;
+}
+
+static int enqueue_slam_groups(ovb_ctx *ctx, int n_groups, int ldH) {
+  const int N = ctx->N, ld = ctx->ldP;
+  double *P = ctx->P[ctx->cur];
+  double *acc = ctx->d_grp_acc;
+  int *flags = (int *)(acc + ctx->cfg.max_state);
+  cudaMemcpyAsync(ctx->P_snap, P, sizeof(double) * (size_t)ld * N, cudaMemcpyDeviceToDevice, ctx->stream);
+  cudaMemsetAsync(acc, 0, sizeof(double) * ((size_t)ctx->cfg.max_state + 4), ctx->stream);
+  int r_total = 0;
+  for (int g = 0; g < n_groups; g++) {
+    const DevGroup &G = ctx->h_grp[g];
+    if (G.rows == 0)
+      continue;
+    const int n = G.n_cols;
+    const int r = compress_system(ctx, ctx->h_opts->o.compress, ctx->d_Hs + (size_t)G.row0 * ldH, G.rows, n, ldH, ctx->d_R, ldH);
+    ovb_launch(ctx, k_group_take_z, dim3((n + 127) / 128), dim3(128), (size_t)0, (const double *)ctx->d_R, ldH, r, n,
+               (const int *)ctx->d_grp[g].col_state, (const double *)acc, ctx->d_w, ctx->d_info);
+    launch_ekf_update(ctx, ctx->d_R, ldH, r, n, false, 1.0, nullptr);
+    ovb_launch(ctx, k_group_accumulate, dim3((N + 255) / 256), dim3(256), (size_t)0, (const double *)ctx->d_dx, acc, N,
+               (const DevUpdateInfo *)ctx->d_info, flags);
+    ctx->n_launch += 8; // take_z, prep, 2 gemm, chol, trsm, downdate, accumulate
+    r_total += r;
+  }
+  if (r_total > 0) {
+    ovb_launch(ctx, k_group_finish, dim3((N + 31) / 32, (N + 7) / 8), dim3(32, 8), (size_t)0, P, ld, N, (const double *)ctx->P_snap,
+               (const double *)acc, ctx->d_dx, ctx->d_info, (const int *)flags);
+  } else {
+    k_fill_zero_dx<<<(N + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_dx, N);
+  }
+  ctx->n_launch += 1;
+  return r_total;
 }
 
 // Per-kernel timing of the update pipeline (bench.py's roofline block): while on, every kernel launched through
@@ -967,6 +1181,13 @@ ovb_status ovb_last_counters(const ovb_ctx *ctx, int64_t out[4]) {
   out[1] = ctx->n_launch_tsqr_level; // of which k_tsqr_level
   out[2] = (int64_t)ctx->last_h2d_bytes;
   out[3] = (int64_t)ctx->last_d2h_bytes;
+  return OVB_OK;
+}
+
+ovb_status ovb_set_slam_unbounded(ovb_ctx *ctx, int enabled) {
+  if (!ctx)
+    return OVB_ERR_ARG;
+  ctx->slam_unbounded = enabled ? 1 : 0;
   return OVB_OK;
 }
 
@@ -1140,7 +1361,7 @@ ovb_status ovb_slam_update(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_
     return st;
   const int F = pk.n_feats;
   ctx->last_pk_valid = 0; // the replay path re-runs MSCKF updates only
-  const int r = enqueue_update(ctx, pk.n_feats, pk.bv, pk.ldH, pk.m_total, pk.n_all, opts->col_order, ctx->ev, true);
+  const int r = enqueue_update(ctx, pk.n_feats, pk.bv, pk.ldH, pk.m_total, pk.n_all, opts->col_order, ctx->ev, true, pk.n_groups);
   OVB_CUDA_CHECK(ctx, cudaGetLastError());
   OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_feat, ctx->d_feat, sizeof(DevFeat) * (size_t)F, cudaMemcpyDeviceToHost, ctx->stream));
   OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_info, ctx->d_info, ctx->info_bytes + sizeof(double) * (size_t)N, cudaMemcpyDeviceToHost,

@@ -30,6 +30,21 @@ struct DevFrame {
   int clone_slot[OVB_MAX_CLONES];
   int cam_ext_slot[OVB_MAX_CAMS];  // -1 when not calibrated
   int cam_intr_slot[OVB_MAX_CAMS]; // -1 when not calibrated
+  const struct DevGroup *groups;   // SLAM update: its column groups (ctx->d_grp), else null
+};
+
+// SLAM update: one column group = a contiguous feature range whose frame columns plus landmark columns fit OVB_MAX_COLS.
+// Its rows are staged in a group-local canonical layout (the frame slots and the group's landmarks in ascending
+// covariance offset), compressed on their own and applied as one step of a sequential EKF update (ovb_slam_update).
+// A batch of at most OVB_MAX_COLS columns is one group whose layout is the batch's canonical layout.
+struct DevGroup {
+  int f0, f1;      // features [f0, f1)
+  int row0, rows;  // staged rows
+  int n_cols;      // group-local canonical columns
+  int n_ent;       // variables of the layout: frame slots and the group's landmarks, ascending covariance offset
+  int ent[OVB_MAX_VARS + OVB_MAX_COLS]; // >= 0: frame slot; < 0: the landmark of feature -1 - ent
+  int col_state[OVB_MAX_COLS];          // covariance index of each group column
+  short col_frame[OVB_MAX_COLS];        // frame canonical column of each group column, -1 for a landmark column
 };
 
 // camera-at-clone poses (update/UpdaterMSCKF.cpp:98-115), filled on the device by k_cam_poses
@@ -58,7 +73,8 @@ struct DevFeat {
   double p_FinG_fej[3]; // Landmark::get_xyz(true) for the global representations
   double sigma_sq;      // per-class pixel noise variance
   double chi2_mult;     // per-class gate multiplier
-  int lm_slot, pad1;    // slot of the landmark's own 3-wide variable
+  int lm_off;           // covariance offset of the landmark's own variable (3 wide, or 1 for ANCHORED_INVERSE_DEPTH_SINGLE)
+  unsigned short lm_col, grp; // first column of the landmark in its column group's layout, and that group
 };
 
 // written by the column-map kernel; read by TSQR re-order, EKF and the host (D2H with the outputs)
@@ -67,7 +83,7 @@ struct DevUpdateInfo {
   int n_feats_used;             // accepted features
   int rows_stacked;             // Σ (2M-3) over accepted features
   int n_order;                  // variables in Hx_order_big
-  int order_slot[OVB_MAX_VARS]; // slot id of each variable in stacked order
+  int order_slot[OVB_MAX_VARS]; // slot id of each variable in stacked order (MSCKF updates)
   int col_state[OVB_MAX_COLS];  // covariance index of each stacked column (order applied)
   int col_canon[OVB_MAX_COLS];  // canonical column each stacked column comes from
   int neg_diag_index;           // EKF: -1 or first negative diagonal
@@ -157,6 +173,12 @@ struct ovb_ctx {
   BlobView last_bv;
   double *P_snap;
   void *d_flush;
+  // SLAM column groups (grown on demand): the group tables, and for batches of several groups the accumulated state
+  // correction [max_state doubles] followed by the failure flags [not_spd, nonfinite] of the sequential EKF update
+  DevGroup *d_grp, *h_grp;
+  int grp_cap;
+  double *d_grp_acc;
+  int slam_unbounded; // ovb_set_slam_unbounded: SLAM batches beyond OVB_MAX_VARS variables (else OVB_ERR_CAPACITY, as before)
   // bookkeeping for bench.py: kernels launched by the last update pipeline, bytes moved by the last ovb_msckf_update
   int n_launch, n_launch_tsqr_level;
   // normal-equations compression (k_gram.cu)
@@ -190,6 +212,8 @@ void launch_feature_system(ovb_ctx *ctx, int n_feats, BlobView bv, int ldH, int 
 // grow the long-track scratch for the tracks of the packed batch (h_feat); slam: the batch is a SLAM update
 ovb_status feature_scratch_reserve(ovb_ctx *ctx, int n_feats, bool slam);
 void launch_column_map(ovb_ctx *ctx, int n_feats, BlobView bv, int rows_drop = 3);
+// SLAM update: counts of the whole batch; full_map: also the column map of the single group's layout (ctx->d_grp[0])
+void launch_column_map_slam(ovb_ctx *ctx, int n_feats, int rows_drop, int lmw, bool full_map);
 // TSQR of A [m x (n+1)] (last column = residual) in place; R (n x (n+1), diag>=0) to Rout with leading dimension ldR
 void launch_tsqr(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR);
 // gather columns of Rin in the order info->col_canon (n_used of them) into Hs scratch and re-triangularise into Rout
