@@ -266,6 +266,10 @@ def load_library(path: str | None = None) -> C.CDLL:
                                     C.POINTER(ovb_feat_out), c_double_p, C.POINTER(ovb_stats)]
     lib.ovb_slam_delayed_init.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts), c_double_p, c_double_p, INIT_CALLBACK,
                                           C.c_void_p, C.POINTER(ovb_feat_out), c_int_p]
+    lib.ovb_slam_update_reps.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_landmarks), c_int_p, C.POINTER(ovb_opts),
+                                         C.POINTER(ovb_feat_out), c_double_p, C.POINTER(ovb_stats)]
+    lib.ovb_slam_delayed_init_reps.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts), c_int_p, c_double_p, c_double_p,
+                                               INIT_CALLBACK, C.c_void_p, C.POINTER(ovb_feat_out), c_int_p]
     lib.ovb_triangulate.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts),
                                     C.POINTER(ovb_feat_out)]
     lib.ovb_feature_jacobians.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts),
@@ -299,7 +303,8 @@ def load_library(path: str | None = None) -> C.CDLL:
 EXPORTED_SYMBOLS = [
     "ovb_create", "ovb_destroy", "ovb_last_error", "ovb_abi_version", "ovb_opts_default", "ovb_cov_set", "ovb_cov_get",
     "ovb_cov_dim", "ovb_cov_get_marginal", "ovb_cov_clone", "ovb_cov_marginalize", "ovb_cov_propagate", "ovb_cov_initialize",
-    "ovb_msckf_update", "ovb_slam_update", "ovb_set_slam_unbounded", "ovb_slam_delayed_init", "ovb_slam_anchor_change", "ovb_ekf_update", "ovb_triangulate", "ovb_feature_jacobians", "ovb_compress", "ovb_compress_gram", "ovb_compress_cholqr2",
+    "ovb_msckf_update", "ovb_slam_update", "ovb_slam_update_reps", "ovb_set_slam_unbounded", "ovb_slam_delayed_init", "ovb_slam_delayed_init_reps",
+    "ovb_slam_anchor_change", "ovb_ekf_update", "ovb_triangulate", "ovb_feature_jacobians", "ovb_compress", "ovb_compress_gram", "ovb_compress_cholqr2",
     "ovb_chi2_quantile95", "ovb_last_stage_ms", "ovb_set_replay", "ovb_msckf_replay", "ovb_last_counters", "ovb_last_host_us", "ovb_set_profile", "ovb_profile_read",
     "ovb_set_stream", "ovb_msckf_shard_compress", "ovb_msckf_shard_compress_range", "ovb_shard_partition", "ovb_msckf_shard_finish",
 ]
@@ -439,13 +444,15 @@ class Engine:
         self._check(st, allow=(OVB_ERR_NEG_DIAG,))
         return st, out, dx, stats
 
-    def slam_update(self, frame: FrameArrays, feats: FeatArrays, landmarks: "LandmarkArrays", opts: ovb_opts):
+    def slam_update(self, frame: FrameArrays, feats: FeatArrays, landmarks: "LandmarkArrays", opts: ovb_opts, feat_rep=None):
+        """feat_rep: one ovb_feat_rep per landmark (Landmark::_feat_representation), or None for opts.feat_rep."""
         out = FeatOut(feats.n_feats)
         dx = np.zeros(self.cov_dim())
         stats = ovb_stats()
         fs, bs, ls, os_ = frame.struct(), feats.struct(), landmarks.struct(), out.struct()
-        st = self.lib.ovb_slam_update(self.h, C.byref(fs), C.byref(bs), C.byref(ls), C.byref(opts), C.byref(os_),
-                                      _ptr(dx, c_double_p), C.byref(stats))
+        reps = None if feat_rep is None else np.ascontiguousarray(feat_rep, dtype=np.int32)
+        st = self.lib.ovb_slam_update_reps(self.h, C.byref(fs), C.byref(bs), C.byref(ls), _ptr(reps, c_int_p), C.byref(opts), C.byref(os_),
+                                           _ptr(dx, c_double_p), C.byref(stats))
         self._check(st, allow=(OVB_ERR_NEG_DIAG,))
         return st, out, dx, stats
 
@@ -453,9 +460,11 @@ class Engine:
         """slam_update accepts batches of more than OVB_MAX_VARS state variables (off by default)"""
         self._check(self.lib.ovb_set_slam_unbounded(self.h, int(enabled)))
 
-    def slam_delayed_init(self, frame: FrameArrays, feats: FeatArrays, opts: ovb_opts, on_init=None, sigma_pix=None, chi2_multipler=None):
+    def slam_delayed_init(self, frame: FrameArrays, feats: FeatArrays, opts: ovb_opts, on_init=None, sigma_pix=None, chi2_multipler=None,
+                          feat_rep=None):
         """UpdaterSLAM::delayed_init in one call. on_init(feat_index, lm_off, dx_new, dx) must apply dx to the caller's state and
-        refresh the arrays of `frame` IN PLACE. Returns (FeatOut, lm_off array)."""
+        refresh the arrays of `frame` IN PLACE. feat_rep: one ovb_feat_rep per feature (its class representation), or None for
+        opts.feat_rep. Returns (FeatOut, lm_off array)."""
         out = FeatOut(feats.n_feats)
         lm_off = np.full(feats.n_feats, -1, dtype=np.int32)
 
@@ -465,8 +474,10 @@ class Engine:
         cb = INIT_CALLBACK(_cb)
         sp = None if sigma_pix is None else np.ascontiguousarray(sigma_pix, dtype=np.float64)
         cm = None if chi2_multipler is None else np.ascontiguousarray(chi2_multipler, dtype=np.float64)
-        self._check(self.lib.ovb_slam_delayed_init(self.h, C.byref(frame.struct()), C.byref(feats.struct()), C.byref(opts), _ptr(sp, c_double_p),
-                                                   _ptr(cm, c_double_p), cb, None, C.byref(out.struct()), _ptr(lm_off, c_int_p)))
+        reps = None if feat_rep is None else np.ascontiguousarray(feat_rep, dtype=np.int32)
+        self._check(self.lib.ovb_slam_delayed_init_reps(self.h, C.byref(frame.struct()), C.byref(feats.struct()), C.byref(opts), _ptr(reps, c_int_p),
+                                                        _ptr(sp, c_double_p), _ptr(cm, c_double_p), cb, None, C.byref(out.struct()),
+                                                        _ptr(lm_off, c_int_p)))
         return out, lm_off
 
     def triangulate(self, frame: FrameArrays, feats: FeatArrays, opts: ovb_opts):

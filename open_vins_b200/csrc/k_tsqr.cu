@@ -762,26 +762,32 @@ void launch_column_map(ovb_ctx *ctx, int n_feats, BlobView bv, int rows_drop) {
 // of the feature). The counts cover the whole batch; full_map (a batch of one column group) also writes the column map of
 // the group's layout exactly as k_column_map does for slots (unused variables last, in canonical order).
 #define CM_MAX_ENT (OVB_MAX_VARS + OVB_MAX_COLS)
+// A landmark in ANCHORED_INVERSE_DEPTH_SINGLE is 1 wide and loses 2 rows to its bearing projection; the others are 3 wide
+// and keep all 2M rows.
+__device__ __forceinline__ int slam_lm_width(const DevFeat &d) { return d.rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE ? 1 : 3; }
+
 __global__ void k_column_map_slam(const DevFrame *__restrict__ fr, const DevOpts *__restrict__ dop, const DevFeat *__restrict__ feats, int n_feats,
-                                  const unsigned char *__restrict__ feat_order, DevUpdateInfo *__restrict__ info, int rows_drop, int lmw,
-                                  int full_map) {
+                                  const unsigned char *__restrict__ feat_order, DevUpdateInfo *__restrict__ info, int full_map) {
   __shared__ unsigned int key[OVB_MAX_VARS];
   __shared__ unsigned int ekey[CM_MAX_ENT];
   __shared__ int order[CM_MAX_ENT];
-  __shared__ int n_used_feats, rows_stacked;
+  __shared__ int n_used_feats, rows_stacked, lm_cols;
   const int tid = threadIdx.x;
   if (tid < OVB_MAX_VARS)
     key[tid] = 0xffffffffu;
   if (tid == 0) {
     n_used_feats = 0;
     rows_stacked = 0;
+    lm_cols = 0;
   }
   __syncthreads();
   for (int f = tid; f < n_feats; f += blockDim.x) {
     if (feats[f].status != OVB_FEAT_OK)
       continue;
+    const int lmw = slam_lm_width(feats[f]);
     atomicAdd(&n_used_feats, 1);
-    atomicAdd(&rows_stacked, 2 * (feats[f].m1 - feats[f].m0) - rows_drop);
+    atomicAdd(&lm_cols, lmw);
+    atomicAdd(&rows_stacked, 2 * (feats[f].m1 - feats[f].m0) - (lmw == 1 ? 2 : 0));
     const unsigned char *ord = feat_order + (size_t)f * (OVB_MAX_VARS + 1);
     int no = ord[0];
     for (int q = 0; q < no; q++)
@@ -798,7 +804,7 @@ __global__ void k_column_map_slam(const DevFrame *__restrict__ fr, const DevOpts
           n_order++;
         }
       info->n_order = n_order + n_used_feats;
-      info->n_used = used_cols + n_used_feats * lmw;
+      info->n_used = used_cols + lm_cols;
       info->n_feats_used = n_used_feats;
       info->rows_stacked = rows_stacked;
       info->neg_diag_index = -1;
@@ -844,13 +850,13 @@ __global__ void k_column_map_slam(const DevFrame *__restrict__ fr, const DevOpts
     for (int i = 0; i < n_ent; i++) {
       const int e = G->ent[i];
       ekey[i] = (unsigned int)c; // ekey is free now: canonical start column
-      c += e >= 0 ? fr->slot_size[e] : lmw;
+      c += e >= 0 ? fr->slot_size[e] : slam_lm_width(feats[-1 - e]);
     }
     int col = 0, used_cols = 0, n_order = 0;
     for (int q = 0; q < n_ent; q++) {
       const int i = order[q], e = G->ent[i];
       const int off = e >= 0 ? fr->slot_off[e] : feats[-1 - e].lm_off;
-      const int sz = e >= 0 ? fr->slot_size[e] : lmw;
+      const int sz = e >= 0 ? fr->slot_size[e] : slam_lm_width(feats[-1 - e]);
       const bool used = e >= 0 ? key[e] != 0xffffffffu : feats[-1 - e].status == OVB_FEAT_OK;
       for (int k = 0; k < sz; k++) {
         info->col_state[col] = off + k;
@@ -872,9 +878,9 @@ __global__ void k_column_map_slam(const DevFrame *__restrict__ fr, const DevOpts
   }
 }
 
-void launch_column_map_slam(ovb_ctx *ctx, int n_feats, int rows_drop, int lmw, bool full_map) {
-  k_column_map_slam<<<1, 256, 0, ctx->stream>>>(ctx->d_frame, ctx->d_opts, ctx->d_feat, n_feats, ovb_feat_order_ptr(ctx), ctx->d_info, rows_drop,
-                                                lmw, full_map ? 1 : 0);
+void launch_column_map_slam(ovb_ctx *ctx, int n_feats, bool full_map) {
+  k_column_map_slam<<<1, 256, 0, ctx->stream>>>(ctx->d_frame, ctx->d_opts, ctx->d_feat, n_feats, ovb_feat_order_ptr(ctx), ctx->d_info,
+                                                full_map ? 1 : 0);
 }
 
 // B[i][q] = Rin[i][col_canon[q]] for q < n_all, B[i][n_all] = Rin[i][n_all] (residual)

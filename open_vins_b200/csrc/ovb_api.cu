@@ -381,11 +381,24 @@ static ovb_status ensure_groups(ovb_ctx *ctx, int n) {
 // next to the frame's columns in OVB_MAX_COLS. A group's layout is its canonical layout, the frame slots and its landmarks
 // in ascending covariance offset (a batch of one group: the batch's canonical layout). Rows are stacked in input order, so
 // a group's rows are contiguous.
-static ovb_status build_groups(ovb_ctx *ctx, int F, int rows_total, int lmw, Packed *pk) {
+static int slam_lm_width(int rep) { return rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE ? 1 : 3; }
+
+static ovb_status build_groups(ovb_ctx *ctx, int F, int rows_total, Packed *pk) {
   const DevFrame *hf = ctx->h_frame;
-  const int per = (OVB_MAX_COLS - hf->n_all) / lmw; // hf->n_all <= 6 OVB_MAX_CLONES + 14 OVB_MAX_CAMS < OVB_MAX_COLS
-  const int G = (F + per - 1) / per;
-  if (per < 1 || G > 0xffff) {
+  const int room = OVB_MAX_COLS - hf->n_all; // hf->n_all <= 6 OVB_MAX_CLONES + 14 OVB_MAX_CAMS < OVB_MAX_COLS
+  // group g = features [f0[g], f0[g+1]): as many landmarks as their widths fit into room
+  std::vector<int> f0;
+  for (int f = 0, acc = 0; f < F; f++) {
+    const int w = slam_lm_width(ctx->h_feat[f].rep);
+    if (f == 0 || acc + w > room) {
+      f0.push_back(f);
+      acc = 0;
+    }
+    acc += w;
+  }
+  const int G = (int)f0.size();
+  f0.push_back(F);
+  if (room < 3 || G > 0xffff) {
     snprintf(ctx->err, sizeof(ctx->err), "SLAM batch of %d landmarks: %d column groups", F, G);
     return OVB_ERR_CAPACITY;
   }
@@ -396,8 +409,8 @@ static ovb_status build_groups(ovb_ctx *ctx, int F, int rows_total, int lmw, Pac
   std::vector<std::pair<int, int>> lms; // (offset, feature)
   for (int g = 0; g < G; g++) {
     DevGroup &gr = ctx->h_grp[g];
-    gr.f0 = g * per;
-    gr.f1 = std::min(F, gr.f0 + per);
+    gr.f0 = f0[g];
+    gr.f1 = f0[g + 1];
     gr.row0 = ctx->h_feat[gr.f0].row0;
     gr.rows = (gr.f1 < F ? ctx->h_feat[gr.f1].row0 : rows_total) - gr.row0;
     lms.clear();
@@ -412,7 +425,7 @@ static ovb_status build_groups(ovb_ctx *ctx, int F, int rows_total, int lmw, Pac
         gr.ent[n_ent++] = -1 - f;
         ctx->h_feat[f].lm_col = (unsigned short)col;
         ctx->h_feat[f].grp = (unsigned short)g;
-        for (int k = 0; k < lmw; k++, col++) {
+        for (int k = 0; k < slam_lm_width(ctx->h_feat[f].rep); k++, col++) {
           gr.col_frame[col] = -1;
           gr.col_state[col] = ctx->h_feat[f].lm_off + k;
         }
@@ -439,12 +452,14 @@ static ovb_status build_groups(ovb_ctx *ctx, int F, int rows_total, int lmw, Pac
 // lm != nullptr: SLAM batch — every feature brings its landmark (a 3-wide state variable, or 1-wide for
 // ANCHORED_INVERSE_DEPTH_SINGLE), rows are NOT nullspace-projected (2M per feature instead of 2M-3), values/anchors come
 // from the landmark. The landmarks are not frame slots: the batch is cut into column groups (DevGroup), contiguous feature
-// ranges whose frame columns plus landmark columns fit OVB_MAX_COLS.
+// ranges whose frame columns plus landmark columns fit OVB_MAX_COLS. lm_rep: each landmark's representation (NULL: all
+// op->feat_rep).
 // per_feature: the call will launch the per-feature kernel (everything but ovb_triangulate), so its scratch is reserved.
 static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_batch *fb, const ovb_opts *op, const ovb_feat_out *given,
-                              Packed *pk, const ovb_landmarks *lm = nullptr, bool per_feature = true) {
+                              Packed *pk, const ovb_landmarks *lm = nullptr, bool per_feature = true, const int32_t *lm_rep = nullptr) {
   if (!fr || !fb || !op)
     return OVB_ERR_ARG;
+  auto rep_of = [&](int f) { return lm_rep ? lm_rep[f] : op->feat_rep; };
   if (lm && (!lm->lm_off || !lm->value || !lm->value_fej))
     return OVB_ERR_ARG;
   if (fr->n_clones < 1 || fr->n_clones > OVB_MAX_CLONES || fr->n_cams < 1 || fr->n_cams > OVB_MAX_CAMS) {
@@ -474,8 +489,6 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
     int off, size, kind, idx;
   }; // kind 0 clone, 1 ext, 2 intr, 3 landmark
   std::vector<SlotRec> slots;
-  const bool lm_single = lm && op->feat_rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE; // 1-wide landmark (inverse depth only)
-  const int lmw = lm_single ? 1 : 3;
   for (int k = 0; k < fr->n_cams; k++) {
     hf->cam_ext_slot[k] = hf->cam_intr_slot[k] = -1;
     if (op->do_calib_camera_pose) {
@@ -532,12 +545,19 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
   hf->groups = nullptr;
   if (col > OVB_MAX_COLS || col + 1 > std::min(OVB_MAX_COLS, ctx->cfg.max_state) + 8)
     return OVB_ERR_CAPACITY;
-  if (lm) { // landmarks: inside the covariance, overlapping neither a frame variable nor each other
+  if (lm) { // landmarks: a known representation, inside the covariance, overlapping neither a frame variable nor each other
+    for (int f = 0; f < fb->n_feats; f++) {
+      hf->lm_w = std::max(hf->lm_w, slam_lm_width(rep_of(f)));
+      if (rep_of(f) < OVB_REP_GLOBAL_3D || rep_of(f) > OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE) {
+        snprintf(ctx->err, sizeof(ctx->err), "landmark %d: representation %d is not an ovb_feat_rep", f, rep_of(f));
+        return OVB_ERR_ARG;
+      }
+    }
     std::vector<std::pair<int, int>> all; // (offset, size)
     for (const SlotRec &r : slots)
       all.push_back({r.off, r.size});
     for (int f = 0; f < fb->n_feats; f++)
-      all.push_back({lm->lm_off[f], lmw});
+      all.push_back({lm->lm_off[f], slam_lm_width(rep_of(f))});
     std::sort(all.begin(), all.end());
     for (size_t s = 0; s < all.size(); s++) {
       if (all[s].first < 0 || all[s].first + all[s].second > ctx->N) {
@@ -586,6 +606,8 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
       return OVB_ERR_CAPACITY;
     }
     d.row0 = row;
+    d.rep = lm ? rep_of(f) : op->feat_rep;
+    const bool lm_single = lm && d.rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE; // 1-wide landmark (inverse depth only)
     if (lm)
       row += lm_single ? (Mf >= 2 ? 2 * Mf - 2 : 0) : 2 * Mf; // UpdaterSLAM.cpp:344-387: all 2M rows kept (SINGLE: 2 projected out)
     else
@@ -650,7 +672,7 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
     if (lm) {
       d.lm_off = lm->lm_off[f];
       d.status = Mf >= (lm_single ? 2 : 1) ? OVB_FEAT_OK : OVB_FEAT_FEW_MEAS; // UpdaterSLAM.cpp:278-290
-      const bool rel = op->feat_rep >= OVB_REP_ANCHORED_3D;
+      const bool rel = d.rep >= OVB_REP_ANCHORED_3D;
       d.anchor_cam = rel && lm->anchor_cam ? lm->anchor_cam[f] : -1;
       d.anchor_clone = rel && lm->anchor_clone ? lm->anchor_clone[f] : -1;
       if (rel && (d.anchor_cam < 0 || d.anchor_cam >= fr->n_cams || d.anchor_clone < 0 || d.anchor_clone >= fr->n_clones)) {
@@ -693,7 +715,7 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
   pk->n_all = col;
   pk->n_groups = 0;
   if (lm) {
-    ovb_status gs = build_groups(ctx, F, row, lmw, pk);
+    ovb_status gs = build_groups(ctx, F, row, pk);
     if (gs != OVB_OK)
       return gs;
     hf->groups = ctx->d_grp;
@@ -846,17 +868,79 @@ ovb_status ovb_feature_jacobians(ovb_ctx *ctx, const ovb_frame *frame, const ovb
   return OVB_OK;
 }
 
+// JacobiRotation::makeGivens(p, q) (Eigen/src/Jacobi/Jacobi.h, real branch): G' [p; q] = [r; 0], r >= 0
+static void make_givens(double p, double q, double &gc, double &gs) {
+  if (q == 0.0) {
+    gc = p < 0.0 ? -1.0 : 1.0;
+    gs = 0.0;
+  } else if (p == 0.0) {
+    gc = 0.0;
+    gs = q < 0.0 ? 1.0 : -1.0;
+  } else if (std::fabs(p) > std::fabs(q)) {
+    const double t = q / p;
+    double u = std::sqrt(1.0 + t * t);
+    if (p < 0.0)
+      u = -u;
+    gc = 1.0 / u;
+    gs = -t * gc;
+  } else {
+    const double t = p / q;
+    double u = std::sqrt(1.0 + t * t);
+    if (q < 0.0)
+      u = -u;
+    gs = -1.0 / u;
+    gc = -t * gs;
+  }
+}
+
+// UpdaterHelper::nullspace_project_inplace (update/UpdaterHelper.cpp:426-454) of the nf columns of Hf (rows x nf, row-major)
+// out of X (rows x w, row-major): the same Givens sweep; the first nf rows of X are then to be dropped.
+static void nullspace_project_host(double *Hf, int nf, double *X, int w, int rows) {
+  for (int n = 0; n < nf; ++n)
+    for (int m = rows - 1; m > n; m--) {
+      double gc, gs;
+      make_givens(Hf[(size_t)(m - 1) * nf + n], Hf[(size_t)m * nf + n], gc, gs);
+      auto rot = [&](double &x, double &y) { // applyOnTheLeft(m - 1, m, G.adjoint())
+        const double x0 = x, y0 = y;
+        x = gc * x0 - gs * y0;
+        y = gs * x0 + gc * y0;
+      };
+      for (int k = n; k < nf; k++)
+        rot(Hf[(size_t)(m - 1) * nf + k], Hf[(size_t)m * nf + k]);
+      for (int k = 0; k < w; k++)
+        rot(X[(size_t)(m - 1) * w + k], X[(size_t)m * w + k]);
+    }
+}
+
 // UpdaterSLAM::delayed_init in one call (see include/ovb200.h). Composition of the staged entry points with the state mean
 // moved by the caller's callback between the features, exactly the reference's sequential structure.
 ovb_status ovb_slam_delayed_init(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_batch *feats, const ovb_opts *opts, const double *sigma_pix,
                                  const double *chi2_multipler, ovb_init_callback on_init, void *user, ovb_feat_out *out, int32_t *lm_off_out) {
+  return ovb_slam_delayed_init_reps(ctx, frame, feats, opts, nullptr, sigma_pix, chi2_multipler, on_init, user, out, lm_off_out);
+}
+
+ovb_status ovb_slam_delayed_init_reps(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_batch *feats, const ovb_opts *opts,
+                                      const int32_t *feat_rep, const double *sigma_pix, const double *chi2_multipler, ovb_init_callback on_init,
+                                      void *user, ovb_feat_out *out, int32_t *lm_off_out) {
   if (!ctx || !frame || !feats || !opts || !out || !out->status || !out->p_FinA || !out->p_FinG || !out->anchor_cam || !out->anchor_clone || !lm_off_out)
     return OVB_ERR_ARG;
-  if (opts->feat_rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE) {
-    snprintf(ctx->err, sizeof(ctx->err), "ovb_slam_delayed_init: the 1-wide SINGLE representation uses the staged route (INTEGRATION.md)");
+  const int F = feats->n_feats;
+  auto rep_of = [&](int f) { return feat_rep ? feat_rep[f] : opts->feat_rep; };
+  // Which representation sizes a SINGLE landmark when the two classes differ (the feature's own, or feat_rep_slam's) has not
+  // been checked against the reference source: a class mix of SINGLE with a 3-wide representation is refused rather than
+  // guessed. Mixes among the 3-wide representations are unaffected.
+  int n_single = 0;
+  for (int f = 0; f < F; f++) {
+    if (rep_of(f) < OVB_REP_GLOBAL_3D || rep_of(f) > OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE) {
+      snprintf(ctx->err, sizeof(ctx->err), "feature %d: representation %d is not an ovb_feat_rep", f, rep_of(f));
+      return OVB_ERR_ARG;
+    }
+    n_single += rep_of(f) == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE ? 1 : 0;
+  }
+  if (n_single > 0 && n_single < F) {
+    snprintf(ctx->err, sizeof(ctx->err), "ovb_slam_delayed_init: ANCHORED_INVERSE_DEPTH_SINGLE mixed with a 3-wide representation in one call");
     return OVB_ERR_ARG;
   }
-  const int F = feats->n_feats;
   for (int f = 0; f < F; f++)
     lm_off_out[f] = -1;
   if (F <= 0)
@@ -895,7 +979,11 @@ ovb_status ovb_slam_delayed_init(ovb_ctx *ctx, const ovb_frame *frame, const ovb
     Hx.assign((size_t)rows * OVB_MAX_COLS, 0.0);
     res.assign((size_t)rows, 0.0);
     int32_t row_off[2], ncols = 0;
-    st = ovb_feature_jacobians(ctx, frame, &v, opts, &o1, 0, Hf.data(), Hx.data(), res.data(), row_off, &ncols, colidx.data(), OVB_MAX_COLS);
+    ovb_opts o_f = *opts;
+    o_f.feat_rep = rep_of(f);
+    const bool single = o_f.feat_rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE;
+    const int lm_size = single ? 1 : 3;
+    st = ovb_feature_jacobians(ctx, frame, &v, &o_f, &o1, 0, Hf.data(), Hx.data(), res.data(), row_off, &ncols, colidx.data(), OVB_MAX_COLS);
     if (st != OVB_OK)
       return st;
     // Hx_order: the variables this feature touches = runs of consecutive covariance columns with a non-zero entry
@@ -921,12 +1009,42 @@ ovb_status ovb_slam_delayed_init(ovb_ctx *ctx, const ovb_frame *frame, const ovb
     for (int i = 0; i < rows; i++)
       for (int j = 0; j < n; j++)
         HR[(size_t)i * n + j] = Hx[(size_t)i * OVB_MAX_COLS + used[(size_t)j]];
+    const double *HL = Hf.data(), *rs = res.data();
+    int r = rows;
+    if (single) {
+      // the SINGLE branch of delayed_init: the stage-0 H_f is that of ANCHORED_MSCKF_INVERSE_DEPTH; its depth column joins the state
+      // columns, [H_x | dz/drho | res] is projected onto the left nullspace of the two bearing columns, and the landmark is
+      // initialised 1 wide from the rows that remain
+      std::vector<double> Hb((size_t)rows * 2), X((size_t)rows * (n + 2));
+      for (int i = 0; i < rows; i++) {
+        Hb[(size_t)i * 2] = Hf[(size_t)i * 3];
+        Hb[(size_t)i * 2 + 1] = Hf[(size_t)i * 3 + 1];
+        for (int j = 0; j < n; j++)
+          X[(size_t)i * (n + 2) + j] = HR[(size_t)i * n + j];
+        X[(size_t)i * (n + 2) + n] = Hf[(size_t)i * 3 + 2];
+        X[(size_t)i * (n + 2) + n + 1] = res[i];
+      }
+      nullspace_project_host(Hb.data(), 2, X.data(), n + 2, rows);
+      r = rows - 2;
+      HR.assign((size_t)r * n, 0.0);
+      Hf.assign((size_t)r, 0.0);
+      res.assign((size_t)r, 0.0);
+      for (int i = 0; i < r; i++) {
+        const double *xi = X.data() + (size_t)(i + 2) * (n + 2);
+        for (int j = 0; j < n; j++)
+          HR[(size_t)i * n + j] = xi[j];
+        Hf[i] = xi[n];
+        res[i] = xi[n + 1];
+      }
+      HL = Hf.data();
+      rs = res.data();
+    }
     const double sp = sigma_pix ? sigma_pix[f] : opts->sigma_pix, cm = chi2_multipler ? chi2_multipler[f] : opts->chi2_multipler;
     const int N0 = ctx->N;
     int accepted = 0;
     double dx_new[3] = {0, 0, 0};
-    dx.assign((size_t)N0 + 3, 0.0);
-    st = ovb_cov_initialize(ctx, off.data(), sz.data(), (int)off.size(), HR.data(), Hf.data(), res.data(), rows, 3, sp * sp, cm, &accepted, dx_new, dx.data());
+    dx.assign((size_t)N0 + lm_size, 0.0);
+    st = ovb_cov_initialize(ctx, off.data(), sz.data(), (int)off.size(), HR.data(), HL, rs, r, lm_size, sp * sp, cm, &accepted, dx_new, dx.data());
     if (st != OVB_OK)
       return st;
     if (!accepted) {
@@ -935,7 +1053,7 @@ ovb_status ovb_slam_delayed_init(ovb_ctx *ctx, const ovb_frame *frame, const ovb
     }
     lm_off_out[f] = N0;
     if (on_init)
-      on_init(user, f, N0, 3, dx_new, dx.data(), N0 + 3); // the host moves its mean and refreshes the frame arrays
+      on_init(user, f, N0, lm_size, dx_new, dx.data(), N0 + lm_size); // the host moves its mean and refreshes the frame arrays
   }
   return OVB_OK;
 }
@@ -1045,8 +1163,7 @@ static int enqueue_update(ovb_ctx *ctx, int F, BlobView bv, int ldH, int m_total
     cudaStream_t main_stream = ctx->stream;
     ctx->stream = ctx->side_stream;
     if (slam) {
-      const bool single = ctx->h_opts->o.feat_rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE;
-      launch_column_map_slam(ctx, F, single ? 2 : 0, single ? 1 : 3, n_groups == 1);
+      launch_column_map_slam(ctx, F, n_groups == 1);
     } else {
       launch_column_map(ctx, F, bv, 3);
     }
@@ -1338,6 +1455,11 @@ ovb_status ovb_msckf_update(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat
 // (landmark block appended, no nullspace projection, per-class noise and gate), then the shared compress + EKF stages.
 ovb_status ovb_slam_update(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_batch *feats, const ovb_landmarks *landmarks,
                            const ovb_opts *opts, ovb_feat_out *out, double *dx, ovb_stats *stats) {
+  return ovb_slam_update_reps(ctx, frame, feats, landmarks, nullptr, opts, out, dx, stats);
+}
+
+ovb_status ovb_slam_update_reps(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_batch *feats, const ovb_landmarks *landmarks,
+                                const int32_t *feat_rep, const ovb_opts *opts, ovb_feat_out *out, double *dx, ovb_stats *stats) {
   if (!ctx || !dx || !landmarks || !opts)
     return OVB_ERR_ARG;
   if (ctx->N < 1) {
@@ -1356,7 +1478,7 @@ ovb_status ovb_slam_update(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_
     return OVB_OK;
   cudaEventRecord(ctx->ev[0], ctx->stream);
   Packed pk;
-  ovb_status st = pack_inputs(ctx, frame, feats, opts, nullptr, &pk, landmarks);
+  ovb_status st = pack_inputs(ctx, frame, feats, opts, nullptr, &pk, landmarks, true, feat_rep);
   if (st != OVB_OK)
     return st;
   const int F = pk.n_feats;
@@ -1803,30 +1925,8 @@ ovb_status ovb_cov_initialize(ovb_ctx *ctx, const int *off, const int *sz, int n
   };
   for (int c0 = 0; c0 < k; ++c0) {
     for (int m = r - 1; m > c0; m--) {
-      // JacobiRotation::makeGivens(p, q) (Eigen/src/Jacobi/Jacobi.h, real branch): G' [p; q] = [r; 0], r >= 0
-      const double p = HL[(size_t)(m - 1) * k + c0], q = HL[(size_t)m * k + c0];
       double gc, gs;
-      if (q == 0.0) {
-        gc = p < 0.0 ? -1.0 : 1.0;
-        gs = 0.0;
-      } else if (p == 0.0) {
-        gc = 0.0;
-        gs = q < 0.0 ? 1.0 : -1.0;
-      } else if (std::fabs(p) > std::fabs(q)) {
-        const double t = q / p;
-        double u = std::sqrt(1.0 + t * t);
-        if (p < 0.0)
-          u = -u;
-        gc = 1.0 / u;
-        gs = -t * gc;
-      } else {
-        const double t = p / q;
-        double u = std::sqrt(1.0 + t * t);
-        if (q < 0.0)
-          u = -u;
-        gs = -1.0 / u;
-        gc = -t * gs;
-      }
+      make_givens(HL[(size_t)(m - 1) * k + c0], HL[(size_t)m * k + c0], gc, gs);
       for (int j = c0; j < k; j++)
         rot(gc, gs, HL[(size_t)(m - 1) * k + j], HL[(size_t)m * k + j]);
       rot(gc, gs, res[m - 1], res[m]);

@@ -31,6 +31,7 @@ struct DevFrame {
   int cam_ext_slot[OVB_MAX_CAMS];  // -1 when not calibrated
   int cam_intr_slot[OVB_MAX_CAMS]; // -1 when not calibrated
   const struct DevGroup *groups;   // SLAM update: its column groups (ctx->d_grp), else null
+  int lm_w;                        // SLAM update: width of the batch's widest landmark (sizes the per-feature kernel's tables)
 };
 
 // SLAM update: one column group = a contiguous feature range whose frame columns plus landmark columns fit OVB_MAX_COLS.
@@ -66,7 +67,8 @@ struct DevFeat {
   int key0, key1;    // camera-key range
   int status;        // ovb_feat_status
   int anchor_cam, anchor_clone;
-  int sched, pad0;   // CTA i of the per-feature kernels works on feature feats[i].sched (longest tracks first)
+  int sched;         // CTA i of the per-feature kernels works on feature feats[i].sched (longest tracks first)
+  int rep;           // SLAM update: the landmark's ovb_feat_rep (Landmark::_feat_representation); unused otherwise
   double p_FinA[3], p_FinG[3];
   double chi2;
   // SLAM update only (landmark already in the state, update/UpdaterSLAM.cpp:333-341, :389-408)
@@ -74,6 +76,7 @@ struct DevFeat {
   double sigma_sq;      // per-class pixel noise variance
   double chi2_mult;     // per-class gate multiplier
   int lm_off;           // covariance offset of the landmark's own variable (3 wide, or 1 for ANCHORED_INVERSE_DEPTH_SINGLE)
+                        // width and rows of a landmark: 3 and 2M, or 1 and 2M-2 for ANCHORED_INVERSE_DEPTH_SINGLE
   unsigned short lm_col, grp; // first column of the landmark in its column group's layout, and that group
 };
 
@@ -212,8 +215,9 @@ void launch_feature_system(ovb_ctx *ctx, int n_feats, BlobView bv, int ldH, int 
 // grow the long-track scratch for the tracks of the packed batch (h_feat); slam: the batch is a SLAM update
 ovb_status feature_scratch_reserve(ovb_ctx *ctx, int n_feats, bool slam);
 void launch_column_map(ovb_ctx *ctx, int n_feats, BlobView bv, int rows_drop = 3);
-// SLAM update: counts of the whole batch; full_map: also the column map of the single group's layout (ctx->d_grp[0])
-void launch_column_map_slam(ovb_ctx *ctx, int n_feats, int rows_drop, int lmw, bool full_map);
+// SLAM update: counts of the whole batch; full_map: also the column map of the single group's layout (ctx->d_grp[0]).
+// Each feature's landmark width and dropped rows follow its DevFeat::rep.
+void launch_column_map_slam(ovb_ctx *ctx, int n_feats, bool full_map);
 // TSQR of A [m x (n+1)] (last column = residual) in place; R (n x (n+1), diag>=0) to Rout with leading dimension ldR
 void launch_tsqr(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR);
 // gather columns of Rin in the order info->col_canon (n_used of them) into Hs scratch and re-triangularise into Rout

@@ -314,17 +314,20 @@ def make_slam_case(n_landmarks=12, n_clones=8, n_cams=2, seed=0, rep=0, calib_ex
                    two_classes=True) -> SlamCase:
     """One UpdaterSLAM::update batch: `n_landmarks` landmarks already in the state (3-wide variables appended after the
     clone window, as State::_variables does), each observed in the newest 1..4 clones; prior P over the augmented state.
-    rep: ovb_feat_rep of all landmarks (global or anchored; the anchor is camera 0 at the track's oldest clone)."""
+    rep: ovb_feat_rep of all landmarks (global or anchored; the anchor is camera 0 at the track's oldest clone), or a sequence of
+    one representation per landmark (widths, offsets, prior sigmas and anchors then follow each landmark)."""
     from .capi import LandmarkArrays
     rng = np.random.default_rng(seed)
     base = make_update_case(n_feats=n_landmarks, n_clones=n_clones, n_cams=n_cams, seed=seed, calib_ext=calib_ext, calib_intr=calib_intr,
                             full_track_frac=1.0, outlier_frac=0.0, degenerate_frac=0.0)
     lay, fr = base.layout, base.frame
     N0 = lay.N
-    lm_size = 1 if rep == 5 else 3  # ANCHORED_INVERSE_DEPTH_SINGLE keeps only the inverse depth in the state
-    N = N0 + lm_size * n_landmarks
-    lm_off = N0 + lm_size * np.arange(n_landmarks)
-    sig = np.concatenate([lay.sigmas(), (0.01 if rep == 5 else 0.05) * np.ones(lm_size * n_landmarks)])
+    reps = [int(rep)] * n_landmarks if np.ndim(rep) == 0 else [int(r) for r in rep]
+    assert len(reps) == n_landmarks
+    lm_size = np.array([1 if r == 5 else 3 for r in reps])  # ANCHORED_INVERSE_DEPTH_SINGLE keeps only the inverse depth in the state
+    N = N0 + int(lm_size.sum())
+    lm_off = N0 + np.concatenate([[0], np.cumsum(lm_size)[:-1]]).astype(np.int64)
+    sig = np.concatenate([lay.sigmas()] + [(0.01 if r == 5 else 0.05) * np.ones(w) for r, w in zip(reps, lm_size)])
     U = rng.standard_normal((N, 12))
     Cn = 0.6 * np.eye(N) + 0.4 * (U @ U.T) / 12
     P = (sig[:, None] * Cn) * sig[None, :]
@@ -334,7 +337,7 @@ def make_slam_case(n_landmarks=12, n_clones=8, n_cams=2, seed=0, rep=0, calib_ex
     keep, meas_off = [], [0]
     first_clone = []
     for f in range(n_landmarks):
-        L = int(rng.integers(max(track_len[0], 2 if rep == 5 else 1), track_len[1] + 1))
+        L = int(rng.integers(max(track_len[0], 2 if reps[f] == 5 else 1), track_len[1] + 1))
         idx = [i for i in range(fa.meas_off[f], fa.meas_off[f + 1]) if fa.clone[i] >= n_clones - L]
         keep += idx
         meas_off.append(meas_off[-1] + len(idx))
@@ -344,12 +347,11 @@ def make_slam_case(n_landmarks=12, n_clones=8, n_cams=2, seed=0, rep=0, calib_ex
     # landmark estimates: truth minus an error of the prior's size; FEJ value = estimate + a small offset
     p_est = base.p_true - 0.03 * rng.standard_normal(base.p_true.shape)
     p_fej = p_est + 2e-3 * rng.standard_normal(p_est.shape)
-    relative = rep in (2, 3, 4, 5)
     anchor_cam = np.full(n_landmarks, -1, dtype=np.int32)
     anchor_clone = np.full(n_landmarks, -1, dtype=np.int32)
     value, value_fej = p_est.copy(), p_fej.copy()
-    if relative:
-        for f in range(n_landmarks):
+    for f in range(n_landmarks):
+        if reps[f] in (2, 3, 4, 5):  # anchored
             c = first_clone[f]
             anchor_cam[f], anchor_clone[f] = 0, c
             to_anchor = lambda pG: fr.cam_R[0] @ (fr.clone_R[c] @ (pG - fr.clone_p[c])) + fr.cam_p[0]

@@ -22,13 +22,13 @@ def _subset(case, a, b):
     return mf.slam_subset(case, a, b)
 
 
-def _time(eng, case, batches, opts, calls, warmup):
+def _time(eng, case, batches, opts, calls, warmup, reps=None):
     per = []
     for it in range(warmup + calls):
         eng.cov_set(case.P)
         tot = 0.0
         for feats, lms in batches:
-            st, out, dx, stats = eng.slam_update(case.frame, feats, lms, opts)
+            st, out, dx, stats = eng.slam_update(case.frame, feats, lms, opts, feat_rep=reps)
             assert st == 0, st
             tot += stats.ms_total
         if it >= warmup:
@@ -47,17 +47,21 @@ def main():
     c4 = sim.make_slam_case(**mf.SLAM4)
     w25 = sim.make_slam_case(n_landmarks=25, n_clones=48, n_cams=8, seed=30, rep=capi.REP_GLOBAL_3D)
     w100 = sim.make_slam_case(n_landmarks=100, n_clones=48, n_cams=8, seed=7, rep=capi.REP_GLOBAL_3D)
+    # every other landmark in the 1-wide ANCHORED_INVERSE_DEPTH_SINGLE, the others in config 4's representation
+    mixed = [capi.REP_ANCHORED_INVERSE_DEPTH_SINGLE if i % 2 else mf.SLAM4["rep"] for i in range(mf.SLAM4["n_landmarks"])]
+    c4m = sim.make_slam_case(**{**mf.SLAM4, "rep": mixed})
     opts = capi.default_opts(feat_rep=capi.REP_GLOBAL_3D, **calib)
     cases = [
         ("config 4, 100 landmarks as 4 calls of 25 (ms per 4 calls)", c4, [_subset(c4, a, b) for a, b in mf.slam_batches(c4)]),
         ("config 4, 100 landmarks in 1 call", c4, [(c4.feats, c4.landmarks)]),
         ("8 cams x 48 clones, calibrated, 25 landmarks in 1 call", w25, [(w25.feats, w25.landmarks)]),
         ("8 cams x 48 clones, calibrated, 100 landmarks in 1 call", w100, [(w100.feats, w100.landmarks)]),
+        ("config 4, 100 landmarks in 1 call, half SINGLE", c4m, [(c4m.feats, c4m.landmarks)], mixed),
     ]
     eng = capi.Engine(max_state=1024, max_feats=256, max_meas=16384)
     eng.set_slam_unbounded()
-    for name, case, batches in cases:
-        ms, stats = _time(eng, case, batches, opts, a.calls, a.warmup)
+    for name, case, batches, *reps in cases:
+        ms, stats = _time(eng, case, batches, opts, a.calls, a.warmup, reps[0] if reps else None)
         print(f"{name:58s} N={case.P.shape[0]:4d} rows={stats.rows_stacked:5d} cols={stats.cols_stacked:4d}  median {1e3 * ms:8.1f} us")
     eng.close()
 
