@@ -387,6 +387,10 @@ ovb_status ovb_msckf_shard_finish(ovb_ctx *ctx, double *stacked_dev, int n_block
 /* out[0] kernels launched by the last update pipeline, out[1] of which TSQR level kernels,
  * out[2]/out[3] bytes copied host->device / device->host by the last ovb_msckf_update. */
 ovb_status ovb_last_counters(const ovb_ctx *ctx, int64_t out[4]);
+/* The last ovb_slam_delayed_init[_reps] call: out[0] features that reached StateHelper::initialize (triangulated), out[1]
+ * stream synchronisations (one for the triangulation, one per such feature), out[2]/out[3] bytes copied host->device /
+ * device->host. */
+ovb_status ovb_last_init_counters(const ovb_ctx *ctx, int64_t out[4]);
 /* Host wall clock (microseconds) of the last ovb_msckf_update: [0] marshalling into the pinned arena + H2D enqueue,
  * [1] kernel and D2H enqueue, [2] wait for the stream, [3] unpacking the results. */
 ovb_status ovb_last_host_us(const ovb_ctx *ctx, double out[4]);

@@ -282,6 +282,7 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.ovb_chi2_quantile95.restype = C.c_double
     lib.ovb_last_stage_ms.argtypes = [vp, C.POINTER(C.c_float * 6)]
     lib.ovb_last_counters.argtypes = [vp, C.POINTER(C.c_int64 * 4)]
+    lib.ovb_last_init_counters.argtypes = [vp, C.POINTER(C.c_int64 * 4)]
     lib.ovb_last_host_us.argtypes = [vp, C.POINTER(C.c_double * 4)]
     lib.ovb_set_stream.argtypes = [vp, C.c_void_p]
     lib.ovb_msckf_shard_compress.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts), C.c_void_p,
@@ -305,7 +306,7 @@ EXPORTED_SYMBOLS = [
     "ovb_cov_dim", "ovb_cov_get_marginal", "ovb_cov_clone", "ovb_cov_marginalize", "ovb_cov_propagate", "ovb_cov_initialize",
     "ovb_msckf_update", "ovb_slam_update", "ovb_slam_update_reps", "ovb_set_slam_unbounded", "ovb_slam_delayed_init", "ovb_slam_delayed_init_reps",
     "ovb_slam_anchor_change", "ovb_ekf_update", "ovb_triangulate", "ovb_feature_jacobians", "ovb_compress", "ovb_compress_gram", "ovb_compress_cholqr2",
-    "ovb_chi2_quantile95", "ovb_last_stage_ms", "ovb_set_replay", "ovb_msckf_replay", "ovb_last_counters", "ovb_last_host_us", "ovb_set_profile", "ovb_profile_read",
+    "ovb_chi2_quantile95", "ovb_last_stage_ms", "ovb_set_replay", "ovb_msckf_replay", "ovb_last_counters", "ovb_last_init_counters", "ovb_last_host_us", "ovb_set_profile", "ovb_profile_read",
     "ovb_set_stream", "ovb_msckf_shard_compress", "ovb_msckf_shard_compress_range", "ovb_shard_partition", "ovb_msckf_shard_finish",
 ]
 
@@ -562,6 +563,13 @@ class Engine:
         a = (C.c_int64 * 4)()
         self._check(self.lib.ovb_last_counters(self.h, C.byref(a)))
         return dict(launches=int(a[0]), tsqr_level_launches=int(a[1]), h2d_bytes=int(a[2]), d2h_bytes=int(a[3]))
+
+    def last_init_counters(self):
+        """Counters of the last slam_delayed_init call: features that reached the initialisation, stream synchronisations,
+        bytes host->device and device->host."""
+        a = (C.c_int64 * 4)()
+        self._check(self.lib.ovb_last_init_counters(self.h, C.byref(a)))
+        return dict(features=int(a[0]), syncs=int(a[1]), h2d_bytes=int(a[2]), d2h_bytes=int(a[3]))
 
     def last_host_us(self):
         """Host wall clock of the last msckf_update in microseconds."""

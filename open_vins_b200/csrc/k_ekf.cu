@@ -399,10 +399,10 @@ __global__ void __launch_bounds__(256) k_ekf_downdate1(double *__restrict__ P, i
   }
 }
 
-__global__ void k_ekf_prep(DevUpdateInfo *info) {
+__global__ void k_ekf_prep(DevUpdateInfo *info, const int *skip) {
   OVB_PDL_ENTER();
   info->neg_diag_index = 0x7fffffff;
-  info->not_spd = 0;
+  info->not_spd = (skip && *skip) ? 1 : 0; // a skipped update takes the failed-factor exits of the kernels below
   info->nonfinite = 0;
 }
 
@@ -410,11 +410,12 @@ __global__ void k_ekf_prep(DevUpdateInfo *info) {
 // d_info->col_state[j]. Everything is enqueued on the context stream; flags land in d_info.
 // gate_only: stop after the Cholesky — d_w then holds w = L^-1 res (|w|^2 = res' S^-1 res) and P is untouched
 // (the Mahalanobis test of StateHelper::initialize, StateHelper.cpp:458-470).
-void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bool gate_only, double sigma2, const double *Rdiag_dev) {
+void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bool gate_only, double sigma2, const double *Rdiag_dev,
+                       const int *skip_dev) {
   const int N = ctx->N;
   const int ld = ctx->ldP;
   double *P = ctx->P[ctx->cur];
-  ovb_launch(ctx, k_ekf_prep, dim3(1), dim3(1), (size_t)(0), ctx->d_info);
+  ovb_launch(ctx, k_ekf_prep, dim3(1), dim3(1), (size_t)(0), ctx->d_info, skip_dev);
   if (r <= 0 || n <= 0)
     return;
   if (!ctx->attr_done[2]) { // function attributes are per device: one flag per context
@@ -483,10 +484,12 @@ void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bo
 //   P[0:N, N:N+k] = -m Hinv',  P[N:N+k, 0:N] = its transpose,  P[N:N+k, N:N+k] = Hinv M Hinv'
 // Single CTA (N <= a few hundred rows, k <= 3): the step is a serial point in the reference as well.
 __global__ void k_cov_init_augment(double *__restrict__ P, int ld, int N, int k, int n, const DevUpdateInfo *__restrict__ info,
-                                   const double *__restrict__ Hx, const double *__restrict__ Hinv, double sigma2) {
+                                   const double *__restrict__ Hx, const double *__restrict__ Hinv, double sigma2, const int *__restrict__ skip) {
   extern __shared__ double ism[]; // m[N][k], then M[k][k]
   double *m = ism, *M = ism + (size_t)N * k;
   const int tid = threadIdx.x;
+  if (skip && *skip)
+    return;
   for (int a = tid; a < N; a += blockDim.x) {
     for (int i = 0; i < k; i++) {
       double acc = 0.0;
@@ -534,7 +537,7 @@ __global__ void k_cov_init_augment(double *__restrict__ P, int ld, int N, int k,
   }
 }
 
-bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, const double *Hinv_dev, double sigma2) {
+bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, const double *Hinv_dev, double sigma2, const int *skip_dev) {
   const int N = ctx->N;
   size_t smem = sizeof(double) * ((size_t)N * k + (size_t)k * k);
   if (smem > 200 * 1024)
@@ -543,8 +546,79 @@ bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, c
     cudaFuncSetAttribute(k_cov_init_augment, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     ctx->attr_done[5] = 1;
   }
-  k_cov_init_augment<<<1, 256, smem, ctx->stream>>>(ctx->P[ctx->cur], ctx->ldP, N, k, n, ctx->d_info, Hx_dev, Hinv_dev, sigma2);
+  k_cov_init_augment<<<1, 256, smem, ctx->stream>>>(ctx->P[ctx->cur], ctx->ldP, N, k, n, ctx->d_info, Hx_dev, Hinv_dev, sigma2, skip_dev);
   return cudaGetLastError() == cudaSuccess;
+}
+
+// ovb_slam_delayed_init, after the per-feature kernel: the head of the init system (status, chi2, skip flag), H_L^-1 of the
+// k x k invertible block by Gauss-Jordan with partial pivoting (the host's order in ovb_cov_initialize), dx_new = H_L^-1 r,
+// and the column map for the augmentation and the EKF update. H_L is rows/columns 3-k..2 of the kernel's 3 x 3 block.
+__global__ void k_init_prep(const DevFeat *__restrict__ feat, DevInitSys *__restrict__ sys, DevUpdateInfo *__restrict__ info, int k, int n) {
+  const int tid = threadIdx.x;
+  const bool ok = feat->status == OVB_FEAT_OK;
+  if (ok)
+    for (int j = tid; j < n; j += blockDim.x)
+      info->col_state[j] = sys->col_state[j];
+  if (tid != 0)
+    return;
+  sys->status = feat->status;
+  sys->chi2 = feat->chi2;
+  int fail = sys->n != n ? 2 : 0;
+  const int o = 3 - k;
+  double A[9], Inv[9];
+  for (int i = 0; i < k; i++)
+    for (int j = 0; j < k; j++) {
+      A[i * k + j] = sys->HL[(o + i) * 3 + o + j];
+      Inv[i * k + j] = (i == j) ? 1.0 : 0.0;
+    }
+  for (int c0 = 0; c0 < k && !fail; c0++) {
+    int piv = c0;
+    for (int i = c0 + 1; i < k; i++)
+      if (fabs(A[i * k + c0]) > fabs(A[piv * k + c0]))
+        piv = i;
+    if (!(fabs(A[piv * k + c0]) > 0.0)) {
+      fail = 1;
+      break;
+    }
+    if (piv != c0)
+      for (int j = 0; j < k; j++) {
+        double t = A[c0 * k + j];
+        A[c0 * k + j] = A[piv * k + j];
+        A[piv * k + j] = t;
+        t = Inv[c0 * k + j];
+        Inv[c0 * k + j] = Inv[piv * k + j];
+        Inv[piv * k + j] = t;
+      }
+    const double d = A[c0 * k + c0];
+    for (int j = 0; j < k; j++) {
+      A[c0 * k + j] /= d;
+      Inv[c0 * k + j] /= d;
+    }
+    for (int i = 0; i < k; i++) {
+      if (i == c0)
+        continue;
+      const double f = A[i * k + c0];
+      for (int j = 0; j < k; j++) {
+        A[i * k + j] -= f * A[c0 * k + j];
+        Inv[i * k + j] -= f * Inv[c0 * k + j];
+      }
+    }
+  }
+  for (int q = 0; q < 3; q++) {
+    double acc = 0.0;
+    if (q < k)
+      for (int i = 0; i < k; i++)
+        acc += Inv[q * k + i] * sys->res[o + i];
+    sys->dx_new[q] = acc;
+  }
+  for (int i = 0; i < k * k; i++)
+    sys->Hinv[i] = Inv[i];
+  sys->fail = ok ? fail : 0;
+  sys->skip = (!ok || fail) ? 1 : 0;
+}
+
+void launch_init_prep(ovb_ctx *ctx, int feat, int k, int n) {
+  k_init_prep<<<1, 256, 0, ctx->stream>>>(ctx->d_feat + feat, ctx->d_init, ctx->d_info, k, n);
 }
 
 // StateHelper::clone: append a copy of the `size`-wide variable at old_off (StateHelper.cpp:371-373)
@@ -655,7 +729,7 @@ __global__ void k_prop_write(double *P, int ld, int N, int new_off, int p, const
 void launch_cov_propagate(ovb_ctx *ctx, int new_off, int p, int q, const int *old_idx_dev, const double *Phi_dev, const double *Q_dev) {
   double *P = ctx->P[ctx->cur];
   int N = ctx->N, ld = ctx->ldP;
-  ovb_launch(ctx, k_ekf_prep, dim3(1), dim3(1), (size_t)(0), ctx->d_info);
+  ovb_launch(ctx, k_ekf_prep, dim3(1), dim3(1), (size_t)(0), ctx->d_info, (const int *)nullptr);
   k_prop_C<<<(N * p + 255) / 256, 256, 0, ctx->stream>>>(P, ld, N, p, q, old_idx_dev, Phi_dev, ctx->d_M, ld);
   k_prop_PCP<<<(p * p + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_M, ld, p, q, old_idx_dev, Phi_dev, Q_dev, ctx->d_S, ld);
   k_prop_write<<<(N * p + 255) / 256, 256, 0, ctx->stream>>>(P, ld, N, new_off, p, ctx->d_M, ld, ctx->d_S, ld, ctx->d_info);

@@ -21,6 +21,7 @@
 //    = 384 measurements) run the BIG algorithm with those blocks in the CTA's global scratch slice as well;
 //  * rows are written straight into the stacked staging matrix in canonical column order, coalesced.
 // Compiled with -fmad=false (see geom.cuh).
+#include <algorithm>
 #include <cstdio>
 #include "geom.cuh"
 #include "chol.cuh"
@@ -253,7 +254,14 @@ __device__ __forceinline__ bool rep_is_relative(int rep) {
 // strides over the rows (up to 2 * OVB_MAX_MEAS_PER_FEAT = 3 * FT_THREADS).
 // LONG runs one CTA per SM (its grid is at most the SM count), so it may use up to 255 registers per thread; ptxas still
 // reports about 300 bytes of spill stores for it (against 1-1.5 KB for the 128-register variants).
-template <bool SLAM, bool BIG, bool LONG = false>
+// INIT (not SLAM): one new landmark of ovb_slam_delayed_init (StateHelper::initialize, UpdaterSLAM.cpp:197-233). The gate is
+// the MSCKF one (the rows orthogonal to all three columns of H_f) with the feature's own representation, sigma and
+// multiplier and the threshold of the initialize system's row count (2M, or 2M-2 for ANCHORED_INVERSE_DEPTH_SINGLE, whose
+// bearing columns the reference projects out before the split). The projected rows go out in the feature's compact
+// columns whatever the gate says, and the top rows Q1'[H_x | H_f | r] of the Householder split (the init system) go to
+// `dump`, a DevInitSys. A Householder split differs from the reference's Givens split by a k x k orthogonal transform of
+// the init rows, which leaves H_L^-1 H_R, H_L^-1 r and the posterior unchanged (tests/test_slam_init_cpu.py).
+template <bool SLAM, bool BIG, bool LONG = false, bool INIT = false>
 __global__ void __launch_bounds__(FT_THREADS, LONG ? 1 : 2)
     k_feature_system(const DevFrame *__restrict__ fr, const DevOpts *__restrict__ dop, DevFeat *__restrict__ feats, int sched_lo, int n_feats,
                      BlobView bv,
@@ -261,6 +269,7 @@ __global__ void __launch_bounds__(FT_THREADS, LONG ? 1 : 2)
                      unsigned char *__restrict__ feat_order, int mode, int maxM, int nblk, double *__restrict__ scratch,
                      size_t scratch_per_cta, double *__restrict__ dump, int ld_dump, int dump_rows) {
   static_assert(BIG || !LONG, "the long-track layout keeps S in scratch");
+  static_assert(!(SLAM && INIT), "a delayed initialisation is not a SLAM update");
   static_assert(2 * OVB_MAX_MEAS_PER_FEAT <= 3 * FT_THREADS, "Householder rows per thread");
   constexpr int RPT = LONG ? 3 : 1; // rows of H_f per thread in the Householder QR
   OVB_PDL_ENTER();
@@ -355,7 +364,7 @@ __global__ void __launch_bounds__(FT_THREADS, LONG ? 1 : 2)
     DevFeat *F = &feats[f];
     // SLAM landmarks kept as a single inverse depth (ANCHORED_INVERSE_DEPTH_SINGLE, UpdaterSLAM.cpp:344-353): the landmark
     // variable is 1 wide (the depth column of H_f) and the two bearing columns are projected out like an MSCKF feature's three
-    const bool single = slam && (F->rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE);
+    const bool single = (SLAM || INIT) && (F->rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE);
     const int nproj = slam ? (single ? 2 : 0) : 3; // columns of H_f that are projected out = rows removed
     const int r0 = nproj;
     const int lmw = single ? 1 : 3;                // width of the landmark block (block 5)
@@ -385,7 +394,7 @@ __global__ void __launch_bounds__(FT_THREADS, LONG ? 1 : 2)
       }
     }
     // SINGLE's Jacobians are those of ANCHORED_MSCKF_INVERSE_DEPTH (UpdaterSLAM.cpp:327-329), as DevOpts::rep remaps MSCKF features
-    const int rep = SLAM ? (single ? OVB_REP_ANCHORED_MSCKF_INVERSE_DEPTH : F->rep) : dop->rep;
+    const int rep = (SLAM || INIT) ? (single ? OVB_REP_ANCHORED_MSCKF_INVERSE_DEPTH : F->rep) : dop->rep;
     const bool relative = rep_is_relative(rep);
     const int acam = F->anchor_cam, aclone = F->anchor_clone;
     const dv3 p_FinA = ld_v3(F->p_FinA);
@@ -817,6 +826,27 @@ __global__ void __launch_bounds__(FT_THREADS, LONG ? 1 : 2)
       Z[2 * (n_all + 1) + j] = z2;
     }
     __syncthreads();
+    if constexpr (INIT) { // H_L = Q1' H_f: the same reflector sweep on the three columns of H_f, rows 0..2
+      double wf9[9];
+#pragma unroll
+      for (int e = 0; e < 9; e++)
+        wf9[e] = 0.0;
+      for (int i = tid; i < rows; i += FT_THREADS) {
+#pragma unroll
+        for (int kq = 0; kq < 3; kq++)
+#pragma unroll
+          for (int c = 0; c < 3; c++)
+            wf9[3 * kq + c] += V[3 * i + kq] * mv.Hf[3 * i + c];
+      }
+      block_sum_n<9>(wf9, red);
+      if (tid < 9) {
+        const int i = tid / 3, c = tid % 3;
+        const double z0 = tau[0] * wf9[c];
+        const double z1 = tau[1] * (wf9[3 + c] - G10 * z0);
+        const double z2 = tau[2] * (wf9[6 + c] - G20 * z0 - G21 * z1);
+        ((DevInitSys *)dump)->HL[3 * i + c] = mv.Hf[3 * i + c] - ((V[3 * i] * z0 + V[3 * i + 1] * z1) + V[3 * i + 2] * z2);
+      }
+    }
 
     const int nr = rows - r0;
     bool spd = true;
@@ -1081,7 +1111,7 @@ __global__ void __launch_bounds__(FT_THREADS, LONG ? 1 : 2)
     }
     const double qnan = __longlong_as_double(0x7ff8000000000000LL);
     double chi2 = spd ? c2 : qnan;
-    double chi2_check = chi2_table[min(nr, OVB_CHI2_TABLE_LEN - 1)];
+    double chi2_check = chi2_table[min(INIT ? (single ? rows - 2 : rows) : nr, OVB_CHI2_TABLE_LEN - 1)];
     bool gated = !(chi2 <= F->chi2_mult * chi2_check); // UpdaterMSCKF.cpp:225, UpdaterSLAM.cpp:409 (NaN rejects)
     if (tid == 0) {
       F->chi2 = chi2;
@@ -1135,6 +1165,36 @@ __global__ void __launch_bounds__(FT_THREADS, LONG ? 1 : 2)
           }
         }
       }
+    } else if constexpr (INIT) {
+      // compact columns c < wf (canonical order of the touched slots), the residual at c = wf. Rows 3.. are the projected
+      // system at row0; rows 3-k..2 the init system (SINGLE drops the two bearing rows 0-1).
+      DevInitSys *sys = (DevInitSys *)dump;
+      const int i0 = single ? 2 : 0;
+      for (int c = tid; c <= wf; c += FT_THREADS) {
+        int s = 0, kk = 0, j = n_all;
+        if (c < wf) {
+          s = lcol_slot[c];
+          kk = lcol_k[c];
+          j = fr->slot_col[s] + kk;
+          sys->col_state[c] = fslot_off[s] + kk;
+        }
+        const double z0 = Z[j], z1 = Z[(n_all + 1) + j], z2 = Z[2 * (n_all + 1) + j];
+        double *out = Hs + (size_t)F->row0 * ldH + c;
+        for (int i = i0; i < rows; i++) {
+          const int I = i >> 1, r = i & 1;
+          const int b = (j == n_all) ? 255 : mv.lut[(size_t)I * mv.lutw + s];
+          const double xv = (j == n_all) ? mv.res[i] : (b == 255 ? 0.0 : mv.blk(I, b)[8 * r + kk]);
+          const double v = xv - ((V[3 * i] * z0 + V[3 * i + 1] * z1) + V[3 * i + 2] * z2);
+          if (i >= 3)
+            out[(size_t)(i - 3) * ldH] = v;
+          else if (c < wf)
+            sys->HR[(size_t)(i - i0) * wf + c] = v;
+          else
+            sys->res[i] = v;
+        }
+      }
+      if (tid == 0)
+        sys->n = wf;
     } else {
       for (int jb = 0; jb <= n_all; jb += FT_THREADS) {
         int j = jb + tid;
@@ -1252,9 +1312,12 @@ static int feature_path(int M, const FeatDims &dm, int nblk) {
   return FT_LONG;
 }
 
-ovb_status feature_scratch_reserve(ovb_ctx *ctx, int n_feats, bool slam) {
+// the delayed initialisation's tracks carry the anchor blocks whatever the call's representation (each feature has its own)
+#define FT_INIT_NBLK 5
+
+ovb_status feature_scratch_reserve(ovb_ctx *ctx, int n_feats, bool slam, bool init) {
   const FeatDims dm = feature_dims(ctx, slam);
-  const int nblk = feature_nblk(ctx, slam);
+  const int nblk = init ? FT_INIT_NBLK : feature_nblk(ctx, slam);
   int n_long = 0, maxM = 0;
   for (int f = 0; f < n_feats; f++) {
     const int M = ctx->h_feat[f].m1 - ctx->h_feat[f].m0;
@@ -1393,4 +1456,32 @@ void launch_feature_system(ovb_ctx *ctx, int n_feats, BlobView bv, int ldH, int 
       cudaEventRecord(joined[s], streams[s]);
       cudaStreamWaitEvent(main_stream, joined[s], 0);
     }
+}
+
+void launch_feature_init(ovb_ctx *ctx, int sched, BlobView bv, int ldH) {
+  const FeatDims dm = feature_dims(ctx, false);
+  const int nblk = FT_INIT_NBLK;
+  if (!ctx->attr_done[6]) {
+    cudaFuncSetAttribute(k_feature_system<false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FT_SMEM_LIMIT);
+    cudaFuncSetAttribute(k_feature_system<false, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FT_SMEM_LIMIT);
+    cudaFuncSetAttribute(k_feature_system<false, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FT_SMEM_LIMIT);
+    ctx->attr_done[6] = 1;
+  }
+  const DevFeat &d = ctx->h_feat[ctx->h_feat[sched].sched];
+  const int cM = std::min(std::max(d.m1 - d.m0, 2), OVB_MAX_MEAS_PER_FEAT);
+  const int path = feature_path(cM, dm, nblk);
+  double *scratch = nullptr;
+  size_t per_cta = ctx->scratch_per_cta;
+  if (path == FT_BIG) {
+    scratch = ctx->d_scratch;
+  } else if (path == FT_LONG) { // feature_scratch_reserve(init) sized d_long for the call's longest track
+    per_cta = feature_long_slice_doubles(cM, dm.n_slots, nblk);
+    scratch = ctx->d_long;
+  }
+  auto kern = path == FT_TILE ? k_feature_system<false, false, false, true>
+                              : (path == FT_BIG ? k_feature_system<false, true, false, true> : k_feature_system<false, true, true, true>);
+  ovb_launch(ctx, kern, dim3(1), dim3(FT_THREADS), feature_smem_bytes(cM, dm, nblk, path), ctx->d_frame, ctx->d_opts, ctx->d_feat, sched, sched + 1,
+             bv, ctx->P[ctx->cur], ctx->ldP, ctx->d_chi2_table, ctx->d_Hs, ldH, nullptr, 0, cM, nblk, scratch, per_cta, (double *)ctx->d_init,
+             0, 0);
+  ctx->n_launch++;
 }

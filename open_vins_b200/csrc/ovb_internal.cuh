@@ -94,6 +94,26 @@ struct DevUpdateInfo {
   int nonfinite;
 };
 
+// ovb_slam_delayed_init: one feature's StateHelper::initialize system on the device. The per-feature kernel's INIT
+// instantiation writes the k init rows (k = 3, or 1 for ANCHORED_INVERSE_DEPTH_SINGLE) and the column map, k_init_prep
+// finishes it; the head (status .. dx_new) is what the host reads back after the feature.
+struct DevInitSys {
+  int status;       // the feature's status after the gate; OVB_FEAT_OK = accepted
+  int skip;         // nonzero: every kernel after the gate leaves P alone (rejected, or one of the failures below)
+  int fail;         // 1: H_L is rank deficient, 2: the kernel's column count differs from the host's
+  int pad;
+  double chi2;
+  double dx_new[3]; // H_L^-1 res_init
+  // ---- written by the per-feature kernel
+  int n;                        // state columns the feature touches (canonical order)
+  int col_state[OVB_MAX_COLS];  // covariance index of each of them
+  double HL[9];                 // Q1' H_f, 3 x 3 (rows 0..2 of the Householder split; SINGLE uses entry [2][2])
+  double res[3];                // Q1' r
+  double HR[3 * OVB_MAX_COLS];  // Q1' H_x, k x n with leading dimension n (the rows SINGLE keeps: row 2 only)
+  double Hinv[9];               // k x k, written by k_init_prep
+};
+#define OVB_INIT_HEAD_BYTES (4 * sizeof(int) + 4 * sizeof(double))
+
 // packed measurement blob layout (device): [meas_off int32 (F+1)][cam u8 (M)][pad][clone u16 (M)][pad][uv f32 2M][uvn f32 2M][keys u8]
 struct BlobView {
   const uint8_t *cam;
@@ -190,6 +210,10 @@ struct ovb_ctx {
   double *d_cqw; // wide systems (k_cholqr.cu): [G1 | G2 | packed diagonal-block factors | scalars]
   size_t cqw_cap;
   size_t last_h2d_bytes, last_d2h_bytes;
+  // ovb_slam_delayed_init: the device system of the current feature and its pinned read-back (allocated on first use), and
+  // the counters of the last call (ovb_last_init_counters)
+  DevInitSys *d_init, *h_init;
+  int64_t init_counters[4];
   // per-kernel profile (ovb_set_profile): CUDA events around every ovb_launch of the main stream; PDL is off while it is on
   int prof_on, prof_n;
   cudaEvent_t prof_ev[2 * 96];
@@ -212,8 +236,15 @@ void launch_triangulate(ovb_ctx *ctx, int n_feats, BlobView bv);
 // mode 2: like 0 but features keep the status/p_FinG given (no triangulation ran) — used by ovb_feature_jacobians
 // Every track runs on the path it fits (shared-memory tile, BIG, or long-track; see k_feature.cu).
 void launch_feature_system(ovb_ctx *ctx, int n_feats, BlobView bv, int ldH, int mode);
-// grow the long-track scratch for the tracks of the packed batch (h_feat); slam: the batch is a SLAM update
-ovb_status feature_scratch_reserve(ovb_ctx *ctx, int n_feats, bool slam);
+// grow the long-track scratch for the tracks of the packed batch (h_feat); slam: the batch is a SLAM update, init: the
+// tracks run through launch_feature_init
+ovb_status feature_scratch_reserve(ovb_ctx *ctx, int n_feats, bool slam, bool init = false);
+// ovb_slam_delayed_init: the per-feature kernel's INIT instantiation for the one feature feats[sched].sched: the gate of
+// StateHelper::initialize with the feature's own sigma / multiplier, its 2M-3 projected rows (compact columns, residual
+// last) at its row0 of d_Hs, and its init system in ctx->d_init
+void launch_feature_init(ovb_ctx *ctx, int sched, BlobView bv, int ldH);
+// finish the init system: H_L^-1, dx_new, the column map into d_info, the skip flag; n = the host's column count
+void launch_init_prep(ovb_ctx *ctx, int feat, int k, int n);
 void launch_column_map(ovb_ctx *ctx, int n_feats, BlobView bv, int rows_drop = 3);
 // SLAM update: counts of the whole batch; full_map: also the column map of the single group's layout (ctx->d_grp[0]).
 // Each feature's landmark width and dropped rows follow its DevFeat::rep.
@@ -235,10 +266,14 @@ bool launch_trsm_rows(ovb_ctx *ctx, double *A, int ldA, int m, int nt, const dou
 bool launch_chol_solve_wide(ovb_ctx *ctx, double *S, int ldS, int r, double *w, double *invdiag, double *M, int ldM, int N, bool gate_only);
 void launch_reorder_R(ovb_ctx *ctx, const double *Rin, int n_all, int ldRin, double *Rout, int ldRout);
 // EKF update from an upper-trapezoidal / dense H [r x n] with column->state map in d_info (device-side sizes)
+// skip_dev (optional): a device flag read after the previous kernels; nonzero marks the update failed before it starts
+// (info->not_spd), so P is left untouched and dx = 0
 void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r_max, int n_max, bool sizes_from_info, double sigma2,
-                       const double *Rdiag_dev);
-// false: the launch was refused (shared-memory footprint) or failed; the caller must not grow N
-bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, const double *Hinv_dev, double sigma2);
+                       const double *Rdiag_dev, const int *skip_dev = nullptr);
+// false: the launch was refused (shared-memory footprint) or failed; the caller must not grow N.
+// skip_dev (optional): the kernel returns without writing when *skip_dev is nonzero
+bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, const double *Hinv_dev, double sigma2,
+                             const int *skip_dev = nullptr);
 void launch_cov_clone(ovb_ctx *ctx, int old_off, int size, const double *dnc_dt_dev, int dt_off);
 void launch_cov_marginalize(ovb_ctx *ctx, int off, int size);
 void launch_cov_propagate(ovb_ctx *ctx, int new_off, int p, int q, const int *old_idx_dev, const double *Phi_dev, const double *Q_dev);
