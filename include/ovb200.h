@@ -296,7 +296,8 @@ ovb_status ovb_set_slam_unbounded(ovb_ctx *ctx, int enabled);
  * columns and the two bearing columns are nullspace-projected out of the system first; the callback's lm_size (dx_new's length)
  * is then 1 and dx has N0 + 1 entries (N0 = ovb_cov_dim() before the landmark), else 3 and N0 + 3.
  * sigma_pix / chi2_multipler: per-feature class values (aruco vs slam options, :225-228) or NULL for ovb_opts'.
- * out->status: OVB_FEAT_OK = initialised, a triangulation status, or OVB_FEAT_CHI2 (gate); lm_off_out[f] = the new landmark's
+ * out->status: OVB_FEAT_OK = initialised, a triangulation status, or OVB_FEAT_CHI2 (gate); out->chi2 (when non-NULL): the
+ * gate's chi2 of every feature that reached it, accepted or rejected, NaN for the others; lm_off_out[f] = the new landmark's
  * covariance id or -1. */
 typedef void (*ovb_init_callback)(void *user, int feat_index, int lm_off, int lm_size, const double *dx_new, const double *dx, int n_dx);
 ovb_status ovb_slam_delayed_init(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_batch *feats, const ovb_opts *opts, const double *sigma_pix,

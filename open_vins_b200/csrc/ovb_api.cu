@@ -1061,6 +1061,8 @@ ovb_status ovb_slam_delayed_init_reps(ovb_ctx *ctx, const ovb_frame *frame, cons
       snprintf(ctx->err, sizeof(ctx->err), "ovb_slam_delayed_init: feature %d touches %d columns, the host counted %d", f, ctx->h_init->n, n);
       return OVB_ERR_CUDA;
     }
+    if (out->chi2) // the gate's value, accepted or rejected (NaN: S was not positive definite)
+      out->chi2[f] = hs->chi2;
     if (hs->status != OVB_FEAT_OK) {
       out->status[f] = hs->status;
       continue;
