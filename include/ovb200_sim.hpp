@@ -21,6 +21,7 @@
 #include <map>
 #include <random>
 #include <sstream>
+#include <stdexcept>
 #include <string>
 #include <unordered_map>
 #include <utility>
@@ -336,19 +337,16 @@ public:
     timestamp = timestamp_last_imu = timestamp_last_cam = spline.get_start_time();
     Mat3 R_GtoI_init;
     Vec3 p_IinG_init;
-    if (!spline.get_pose(timestamp, R_GtoI_init, p_IinG_init)) {
-      std::fprintf(stderr, "[SIM]: unable to find the first pose in the spline\n");
-      std::exit(EXIT_FAILURE);
-    }
+    // the reference exits the process here; throwing lets a runner that holds several simulations report the failing one
+    if (!spline.get_pose(timestamp, R_GtoI_init, p_IinG_init))
+      throw std::runtime_error("[SIM]: unable to find the first pose in the spline");
     // find the timestamp at which we have moved enough (:76-109)
     double distance = 0.0;
     while (true) {
       Mat3 R_GtoI;
       Vec3 p_IinG;
-      if (!spline.get_pose(timestamp, R_GtoI, p_IinG)) {
-        std::fprintf(stderr, "[SIM]: unable to find jolt in the groundtruth data to initialize at\n");
-        std::exit(EXIT_FAILURE);
-      }
+      if (!spline.get_pose(timestamp, R_GtoI, p_IinG))
+        throw std::runtime_error("[SIM]: unable to find jolt in the groundtruth data to initialize at");
       distance += norm(p_IinG - p_IinG_init);
       p_IinG_init = p_IinG;
       if (distance > params.sim_distance_threshold)

@@ -82,7 +82,8 @@ def build_sim_tools(force: bool = False) -> str:
     cxx = os.environ.get("CXX", "g++")
     exe = os.path.join(HERE, "ovb_run_simulation")
     if force or _stale(exe, [src, OUT] + hdrs):
-        subprocess.check_call([cxx, "-std=c++17", "-O2", "-Wall", "-DOVB_SIM_ENGINE", "-I", inc, src, "-L", HERE, "-lovb200", "-Wl,-rpath,$ORIGIN", "-o", exe])
+        subprocess.check_call([cxx, "-std=c++17", "-O2", "-Wall", "-pthread", "-DOVB_SIM_ENGINE", "-I", inc, src, "-L", HERE, "-lovb200", "-Wl,-rpath,$ORIGIN",
+                               "-o", exe])
     return exe
 
 

@@ -1295,12 +1295,16 @@ int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, doub
   if (!cq_ensure_G(ctx))
     return -1;
   if (need_part > ctx->Gpart_cap) {
+    // the stacked rows grow over a run's first ~30 updates; taking half as much again keeps regrowth to a few early
+    // updates (cudaFree waits for the whole device, other contexts' work included: tools/monte_carlo_timing.py)
+    const size_t cap = need_part + need_part / 2;
     if (ctx->d_Gpart)
       cudaFree(ctx->d_Gpart);
     ctx->d_Gpart = nullptr;
-    if (cudaMalloc(&ctx->d_Gpart, sizeof(double) * need_part) != cudaSuccess)
+    ctx->Gpart_cap = 0;
+    if (cudaMalloc(&ctx->d_Gpart, sizeof(double) * cap) != cudaSuccess)
       return -1;
-    ctx->Gpart_cap = need_part;
+    ctx->Gpart_cap = cap;
   }
   double *G = ctx->d_G, *L1 = G + (size_t)ldW * ldW, *L2 = L1 + (size_t)ldW * ldW;
   static_assert(CQ_PK_DOUBLES <= (CQ_MAXN + 8) * (CQ_MAXN + 8), "packed factor must fit its slot");

@@ -22,16 +22,28 @@ CASE_CONFIG2 = os.path.join(os.path.dirname(HERE), "tests", "golden", "rpng_sim_
 
 
 def run(exe=None, traj=None, cams=2, clones=11, msckf=10, pts=250, frames=0, calib=1, est=None, timing=None, capture=None, integration="rk4",
-        compress="cholqr2", timeout=1800):
-    """Runs the simulation; returns the parsed JSON summary. capture = (frame_index, path_prefix) dumps that update's inputs."""
+        compress="cholqr2", seed_init=0, seed_perturb=0, seed_meas=0, runs=None, jobs=None, out_dir=None, timeout=1800):
+    """Runs the simulation; returns the parsed JSON summary. capture = (frame_index, path_prefix) dumps that update's inputs.
+    seed_init / seed_perturb / seed_meas: the simulator's random seeds (rpng_sim's sim_seed_state_init, sim_seed_preturb,
+    sim_seed_measurements). runs = K: a Monte-Carlo batch in one process, run r with measurement seed seed_meas + r, on
+    `jobs` host threads (default min(K, hardware threads)); out_dir receives est_<seed>.txt per run and, when `timing` is
+    truthy, timing_<seed>.csv. The batch summary lists every run under "per_run" with the mean and population standard
+    deviation of both ATEs."""
     cmd = [exe or ENGINE_EXE, "--traj", traj or TRAJ_FIXTURE, "--cams", str(cams), "--clones", str(clones), "--msckf", str(msckf), "--pts", str(pts),
-           "--frames", str(frames), "--calib", str(int(calib)), "--integration", integration, "--compress", compress]
+           "--frames", str(frames), "--calib", str(int(calib)), "--integration", integration, "--compress", compress,
+           "--seed-init", str(seed_init), "--seed-perturb", str(seed_perturb), "--seed-meas", str(seed_meas)]
     if est:
         cmd += ["--est", est]
     if timing:
-        cmd += ["--timing", timing]
+        cmd += ["--timing"] if runs else ["--timing", timing]
     if capture:
         cmd += ["--capture", str(capture[0]), capture[1]]
+    if runs:
+        cmd += ["--runs", str(runs)]
+        if jobs:
+            cmd += ["--jobs", str(jobs)]
+        if out_dir:
+            cmd += ["--out-dir", str(out_dir)]
     out = subprocess.run(cmd, check=True, capture_output=True, text=True, timeout=timeout)
     return json.loads(out.stdout.strip().splitlines()[-1])
 
