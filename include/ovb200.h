@@ -222,6 +222,22 @@ ovb_status ovb_cov_marginalize(ovb_ctx *ctx, int off, int size);
  * Phi is p×q row-major, Q is p×p row-major.                                       state/StateHelper.cpp:36-114 */
 ovb_status ovb_cov_propagate(ovb_ctx *ctx, int new_off, int p, const int *old_off, const int *old_sz, int nold,
                              const double *Phi, const double *Q);
+/* Propagator::propagate_and_clone, covariance side (state/Propagator.cpp:83-137), in one call. For s = 0..steps-1, in this
+ * order and with the reference's arithmetic:
+ *   Qd_s = sym(G_s diag(qc_s[k/3]) G_s')           (Propagator.cpp:453-464; sym(X) = 0.5 (X + X'))
+ *   Phi  = F_s Phi,   Q = sym(F_s Q F_s' + Qd_s)    (Phi = I, Q = 0 before step 0; :83-99)
+ * then StateHelper::EKFPropagation of [new_off, new_off+n) from the variables (old_off[i], old_sz[i]) (:130; their sizes
+ * add up to n), then StateHelper::augment_clone: clone clone_size rows/cols at clone_off, with the time-offset term when
+ * dnc_dt != NULL (:137).
+ * F: [steps][n][n], G: [steps][n][12], qc: [steps][4] (sigma^2/dt of n_w, n_a, n_wb, n_ab), row-major. steps = 0 is legal
+ * (F, G, qc may then be NULL). Phi_out / Q_out (n*n each) may be NULL.
+ * Phi, Q and P are bit-identical to the host loop followed by ovb_cov_propagate and ovb_cov_clone. OVB_ERR_ARG for
+ * malformed arguments and OVB_ERR_CAPACITY for n > 64 or a clone beyond max_state, with P and N untouched;
+ * OVB_ERR_NEG_DIAG when the propagated diagonal goes negative: P then holds the propagated values and nothing is cloned. */
+ovb_status ovb_cov_propagate_imu(ovb_ctx *ctx, int n, int steps, const double *F, const double *G, const double *qc,
+                                 int new_off, const int *old_off, const int *old_sz, int nold,
+                                 int clone_off, int clone_size, const double *dnc_dt, int dt_off,
+                                 double *Phi_out, double *Q_out);
 
 /* StateHelper::initialize + initialize_invertible (state/StateHelper.cpp:393-577): add a NEW `new_size`-wide variable (a SLAM
  * landmark in UpdaterSLAM::delayed_init, update/UpdaterSLAM.cpp:233) at the END of the covariance from the linear system

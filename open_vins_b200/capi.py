@@ -254,6 +254,8 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.ovb_cov_clone.argtypes = [vp, C.c_int, C.c_int, c_double_p, C.c_int]
     lib.ovb_cov_marginalize.argtypes = [vp, C.c_int, C.c_int]
     lib.ovb_cov_propagate.argtypes = [vp, C.c_int, C.c_int, c_int_p, c_int_p, C.c_int, c_double_p, c_double_p]
+    lib.ovb_cov_propagate_imu.argtypes = [vp, C.c_int, C.c_int, c_double_p, c_double_p, c_double_p, C.c_int, c_int_p, c_int_p, C.c_int,
+                                          C.c_int, C.c_int, c_double_p, C.c_int, c_double_p, c_double_p]
     lib.ovb_msckf_update.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts),
                                      C.POINTER(ovb_feat_out), c_double_p, C.POINTER(ovb_stats)]
     lib.ovb_ekf_update.argtypes = [vp, c_int_p, c_int_p, C.c_int, c_double_p, C.c_int, c_double_p, C.c_double,
@@ -303,7 +305,7 @@ def load_library(path: str | None = None) -> C.CDLL:
 
 EXPORTED_SYMBOLS = [
     "ovb_create", "ovb_destroy", "ovb_last_error", "ovb_abi_version", "ovb_opts_default", "ovb_cov_set", "ovb_cov_get",
-    "ovb_cov_dim", "ovb_cov_get_marginal", "ovb_cov_clone", "ovb_cov_marginalize", "ovb_cov_propagate", "ovb_cov_initialize",
+    "ovb_cov_dim", "ovb_cov_get_marginal", "ovb_cov_clone", "ovb_cov_marginalize", "ovb_cov_propagate", "ovb_cov_propagate_imu", "ovb_cov_initialize",
     "ovb_msckf_update", "ovb_slam_update", "ovb_slam_update_reps", "ovb_set_slam_unbounded", "ovb_slam_delayed_init", "ovb_slam_delayed_init_reps",
     "ovb_slam_anchor_change", "ovb_ekf_update", "ovb_triangulate", "ovb_feature_jacobians", "ovb_compress", "ovb_compress_gram", "ovb_compress_cholqr2",
     "ovb_chi2_quantile95", "ovb_last_stage_ms", "ovb_set_replay", "ovb_msckf_replay", "ovb_last_counters", "ovb_last_init_counters", "ovb_last_host_us", "ovb_set_profile", "ovb_profile_read",
@@ -414,6 +416,29 @@ class Engine:
         return self._check(self.lib.ovb_cov_propagate(self.h, new_off, Phi.shape[0], _ptr(old_off, c_int_p),
                                                       _ptr(old_sz, c_int_p), len(old_off), _ptr(Phi, c_double_p),
                                                       _ptr(Q, c_double_p)), allow=(OVB_ERR_NEG_DIAG,))
+
+    def cov_propagate_imu(self, F, G, qc, new_off, old_off, old_sz, clone_off, clone_size, dnc_dt=None, dt_off=-1):
+        """ovb_cov_propagate_imu: F [steps, n, n], G [steps, n, 12], qc [steps, 4]. Returns (status, Phi, Q); OVB_ERR_NEG_DIAG is
+        returned, not raised (P then holds the propagated values and nothing was cloned)."""
+        F = np.ascontiguousarray(F, dtype=np.float64)
+        G = np.ascontiguousarray(G, dtype=np.float64)
+        qc = np.ascontiguousarray(qc, dtype=np.float64)
+        if F.ndim != 3 or F.shape[1] != F.shape[2] or G.shape != (F.shape[0], F.shape[1], 12) or qc.shape != (F.shape[0], 4):
+            raise ValueError(f"F [steps, n, n], G [steps, n, 12], qc [steps, 4] expected, got {F.shape}, {G.shape}, {qc.shape}")
+        steps, n = F.shape[0], F.shape[1]
+        old_off = np.ascontiguousarray(old_off, dtype=np.int32)
+        old_sz = np.ascontiguousarray(old_sz, dtype=np.int32)
+        if old_off.shape != old_sz.shape or old_off.ndim != 1:
+            raise ValueError("old_off and old_sz must be 1-D and of the same length")
+        d = None if dnc_dt is None else np.ascontiguousarray(dnc_dt, dtype=np.float64)
+        if d is not None and d.shape != (int(clone_size),):
+            raise ValueError(f"dnc_dt must hold clone_size = {clone_size} values, got shape {d.shape}")
+        Phi, Q = np.zeros((n, n)), np.zeros((n, n))
+        st = self.lib.ovb_cov_propagate_imu(self.h, n, steps, _ptr(F, c_double_p), _ptr(G, c_double_p), _ptr(qc, c_double_p), int(new_off),
+                                            _ptr(old_off, c_int_p), _ptr(old_sz, c_int_p), len(old_off), int(clone_off), int(clone_size),
+                                            _ptr(d, c_double_p), int(dt_off), _ptr(Phi, c_double_p), _ptr(Q, c_double_p))
+        self._check(st, allow=(OVB_ERR_NEG_DIAG,))
+        return st, Phi, Q
 
     def cov_initialize(self, off, sz, H_R, H_L, res, sigma2=1.0, chi2_mult=1.0):
         """StateHelper::initialize: returns (status, accepted, dx_new[k], dx[N after the call])."""

@@ -622,10 +622,11 @@ void launch_init_prep(ovb_ctx *ctx, int feat, int k, int n) {
 }
 
 // StateHelper::clone: append a copy of the `size`-wide variable at old_off (StateHelper.cpp:371-373)
-__global__ void k_cov_clone(double *P, int ld, int N, int old_off, int size) {
+// neg_diag (optional): the flag of a propagation enqueued before; a negative diagonal there cancels the clone
+__global__ void k_cov_clone(double *P, int ld, int N, int old_off, int size, const int *neg_diag) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   int N2 = N + size;
-  if (idx >= N2 * size)
+  if (idx >= N2 * size || (neg_diag && *neg_diag != 0x7fffffff))
     return;
   int i = idx / size, j = idx % size; // element (i, N+j) and its mirror (N+j, i)
   double v;
@@ -639,30 +640,30 @@ __global__ void k_cov_clone(double *P, int ld, int N, int old_off, int size) {
     P[(size_t)(N + j) * ld + i] = vr;
 }
 // augment_clone time-offset term, step 1: P[:, N..N+size) += P[:, dt] dnc'   (StateHelper.cpp:611-612)
-__global__ void k_cov_dt_cols(double *P, int ld, int N2, int new_off, int size, int dt_off, const double *dnc) {
+__global__ void k_cov_dt_cols(double *P, int ld, int N2, int new_off, int size, int dt_off, const double *dnc, const int *neg_diag) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= N2 * size)
+  if (idx >= N2 * size || (neg_diag && *neg_diag != 0x7fffffff))
     return;
   int i = idx / size, j = idx % size;
   P[(size_t)i * ld + new_off + j] += P[(size_t)i * ld + dt_off] * dnc[j];
 }
 // step 2: P[N..N+size, :] += dnc P[dt, :]   (StateHelper.cpp:613-614) — reads the row written by step 1
-__global__ void k_cov_dt_rows(double *P, int ld, int N2, int new_off, int size, int dt_off, const double *dnc) {
+__global__ void k_cov_dt_rows(double *P, int ld, int N2, int new_off, int size, int dt_off, const double *dnc, const int *neg_diag) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= N2 * size)
+  if (idx >= N2 * size || (neg_diag && *neg_diag != 0x7fffffff))
     return;
   int i = idx / N2, j = idx % N2;
   P[(size_t)(new_off + i) * ld + j] += dnc[i] * P[(size_t)dt_off * ld + j];
 }
 
-void launch_cov_clone(ovb_ctx *ctx, int old_off, int size, const double *dnc_dt_dev, int dt_off) {
+void launch_cov_clone(ovb_ctx *ctx, int old_off, int size, const double *dnc_dt_dev, int dt_off, const int *neg_diag_dev) {
   double *P = ctx->P[ctx->cur];
   int N = ctx->N, N2 = N + size;
   int tot = N2 * size;
-  k_cov_clone<<<(tot + 255) / 256, 256, 0, ctx->stream>>>(P, ctx->ldP, N, old_off, size);
+  k_cov_clone<<<(tot + 255) / 256, 256, 0, ctx->stream>>>(P, ctx->ldP, N, old_off, size, neg_diag_dev);
   if (dnc_dt_dev) {
-    k_cov_dt_cols<<<(tot + 255) / 256, 256, 0, ctx->stream>>>(P, ctx->ldP, N2, N, size, dt_off, dnc_dt_dev);
-    k_cov_dt_rows<<<(tot + 255) / 256, 256, 0, ctx->stream>>>(P, ctx->ldP, N2, N, size, dt_off, dnc_dt_dev);
+    k_cov_dt_cols<<<(tot + 255) / 256, 256, 0, ctx->stream>>>(P, ctx->ldP, N2, N, size, dt_off, dnc_dt_dev, neg_diag_dev);
+    k_cov_dt_rows<<<(tot + 255) / 256, 256, 0, ctx->stream>>>(P, ctx->ldP, N2, N, size, dt_off, dnc_dt_dev, neg_diag_dev);
   }
 }
 
@@ -733,4 +734,105 @@ void launch_cov_propagate(ovb_ctx *ctx, int new_off, int p, int q, const int *ol
   k_prop_C<<<(N * p + 255) / 256, 256, 0, ctx->stream>>>(P, ld, N, p, q, old_idx_dev, Phi_dev, ctx->d_M, ld);
   k_prop_PCP<<<(p * p + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_M, ld, p, q, old_idx_dev, Phi_dev, Q_dev, ctx->d_S, ld);
   k_prop_write<<<(N * p + 255) / 256, 256, 0, ctx->stream>>>(P, ld, N, new_off, p, ctx->d_M, ld, ctx->d_S, ld, ctx->d_info);
+}
+
+// Propagator::propagate_and_clone's accumulation over the IMU steps (Propagator.cpp:83-99, Qd of each step :453-464), in
+// one CTA with Phi, Q and the temporaries in shared memory. For s = 0..steps-1:
+//   Qd  = sym(G_s diag(qc_s[k/3]) G_s')       Phi = F_s Phi       Q = sym(F_s Q F_s' + Qd)        (sym(X) = 0.5 (X + X'))
+// Bit-identical to the host loop of include/ovb200_vio.hpp: every entry is one dot product over ascending k from 0.0 with
+// separate multiply and add, as the host computes it (__dmul_rn / __dadd_rn keep -fmad out of it), and the dense F keeps
+// its zero terms so signed zeros agree too. The symmetrisations are computed by the owner of each pair (i <= j), which
+// writes both halves: 0.5 (x + y) does not depend on the order of x and y.
+// Step s+1's F / G / qc are staged with cp.async while step s computes. Phi and Q go to Phi_out / Q_out (n x n).
+#define PA_THREADS 1024
+
+__device__ __forceinline__ void pa_stage(double *dst, const double *src, int count, int tid) {
+  for (int e = tid; e < count; e += PA_THREADS) {
+    const unsigned d = (unsigned)__cvta_generic_to_shared(dst + e);
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(d), "l"(src + e) : "memory");
+  }
+}
+
+__global__ void __launch_bounds__(PA_THREADS) k_prop_accumulate(int n, int steps, const double *__restrict__ F, const double *__restrict__ G,
+                                                                const double *__restrict__ qc, double *__restrict__ Phi_out,
+                                                                double *__restrict__ Q_out) {
+  extern __shared__ double pa_sm[];
+  const int tid = threadIdx.x, nn = n * n, rec = nn + 12 * n + 4, npairs = n * (n + 1) / 2;
+  double *Phi = pa_sm, *Phi2 = Phi + nn, *Q = Phi2 + nn, *T = Q + nn, *stg = T + nn; // stg: two records [F nn | G 12n | qc 4]
+  unsigned char *pi = (unsigned char *)(stg + 2 * rec), *pj = pi + npairs;         // the pairs i <= j, row by row
+  for (int e = tid; e < nn; e += PA_THREADS) {
+    Phi[e] = (e / n == e % n) ? 1.0 : 0.0;
+    Q[e] = 0.0;
+  }
+  if (tid < n)
+    for (int j = tid, t = tid * n - tid * (tid - 1) / 2; j < n; j++, t++)
+      pi[t] = (unsigned char)tid, pj[t] = (unsigned char)j;
+  auto stage = [&](int s) {
+    double *r = stg + (s & 1) * rec;
+    pa_stage(r, F + (size_t)s * nn, nn, tid);
+    pa_stage(r + nn, G + (size_t)s * 12 * n, 12 * n, tid);
+    pa_stage(r + nn + 12 * n, qc + (size_t)s * 4, 4, tid);
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  if (steps > 0)
+    stage(0);
+  for (int s = 0; s < steps; s++) {
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    __syncthreads(); // step s's record has landed; step s-1 is done with Phi, Q and the other record
+    if (s + 1 < steps)
+      stage(s + 1);
+    const double *f = stg + (s & 1) * rec, *g = f + nn, *w = g + 12 * n;
+    // T = F Q, Phi2 = F Phi
+    for (int e = tid; e < 2 * nn; e += PA_THREADS) {
+      const bool phi = e >= nn;
+      const int ee = phi ? e - nn : e, i = ee / n, j = ee % n;
+      const double *B = phi ? Phi : Q;
+      double acc = 0.0;
+      for (int k = 0; k < n; k++)
+        acc = __dadd_rn(acc, __dmul_rn(f[i * n + k], B[k * n + j]));
+      (phi ? Phi2 : T)[ee] = acc;
+    }
+    __syncthreads();
+    // Q = sym(T F' + Qd), Qd = sym(Qt), Qt = G diag(qc) G'
+    for (int t = tid; t < npairs; t += PA_THREADS) {
+      const int i = pi[t], j = pj[t];
+      double qij = 0.0, qji = 0.0, tij = 0.0, tji = 0.0;
+      for (int k = 0; k < 12; k++) {
+        qij = __dadd_rn(qij, __dmul_rn(__dmul_rn(g[i * 12 + k], w[k / 3]), g[j * 12 + k]));
+        qji = __dadd_rn(qji, __dmul_rn(__dmul_rn(g[j * 12 + k], w[k / 3]), g[i * 12 + k]));
+      }
+      for (int k = 0; k < n; k++) {
+        tij = __dadd_rn(tij, __dmul_rn(T[i * n + k], f[j * n + k]));
+        tji = __dadd_rn(tji, __dmul_rn(T[j * n + k], f[i * n + k]));
+      }
+      const double qd = __dmul_rn(0.5, __dadd_rn(qij, qji));
+      const double v = __dmul_rn(0.5, __dadd_rn(__dadd_rn(tij, qd), __dadd_rn(tji, qd)));
+      Q[i * n + j] = v;
+      Q[j * n + i] = v;
+    }
+    double *x = Phi;
+    Phi = Phi2, Phi2 = x;
+  }
+  __syncthreads();
+  for (int e = tid; e < nn; e += PA_THREADS) {
+    Phi_out[e] = Phi[e];
+    Q_out[e] = Q[e];
+  }
+}
+
+static size_t prop_accumulate_smem(int n) {
+  const size_t nn = (size_t)n * n;
+  return sizeof(double) * (4 * nn + 2 * (nn + 12 * (size_t)n + 4)) + (size_t)n * (n + 1);
+}
+
+bool launch_prop_accumulate(ovb_ctx *ctx, int n, int steps, const double *F_dev, const double *G_dev, const double *qc_dev, double *Phi_dev,
+                            double *Q_dev) {
+  const size_t smem = prop_accumulate_smem(n);
+  if (!ctx->attr_done[7]) {
+    if (cudaFuncSetAttribute(k_prop_accumulate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop_accumulate_smem(OVB_PROP_MAX_N)) != cudaSuccess)
+      return false;
+    ctx->attr_done[7] = 1;
+  }
+  k_prop_accumulate<<<1, PA_THREADS, smem, ctx->stream>>>(n, steps, F_dev, G_dev, qc_dev, Phi_dev, Q_dev);
+  return cudaGetLastError() == cudaSuccess;
 }

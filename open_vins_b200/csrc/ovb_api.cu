@@ -171,6 +171,10 @@ ovb_status ovb_create(const ovb_config *cfg, ovb_ctx **out) {
   CK(cudaMalloc(&ctx->d_scratch, sizeof(double) * ctx->scratch_per_cta * ctx->scratch_ctas));
   ctx->dump_cap = 0;
   ctx->d_dump = nullptr; // allocated on first use by ovb_feature_jacobians(stage 0)
+  // ovb_cov_propagate_imu staging: OVB_PROP_STEPS_RESERVE IMU steps of the 39-wide IMU block (400 Hz IMU, 10 Hz camera: ~41)
+  ctx->imu_cap = (size_t)OVB_PROP_STEPS_RESERVE * (39 * 39 + 12 * 39 + 4) + 64 + 39;
+  CK(cudaMalloc(&ctx->d_imu, sizeof(double) * ctx->imu_cap));
+  CK(cudaMallocHost(&ctx->h_imu, sizeof(double) * ctx->imu_cap));
 #undef CK
   *out = ctx;
   return OVB_OK;
@@ -188,11 +192,11 @@ void ovb_destroy(ovb_ctx *ctx) {
     cudaStreamSynchronize(ctx->stream);
   void *dev[] = {ctx->P[0],   ctx->P[1], ctx->d_arena, ctx->d_cc, ctx->d_feat_order, ctx->d_info, ctx->d_chi2_table, ctx->d_Hs, ctx->d_W[0],
                  ctx->d_W[1], ctx->d_R,  ctx->d_R2,    ctx->d_M,  ctx->d_S,          ctx->d_Y,    ctx->d_w,          ctx->d_scratch,
-                 ctx->d_long, ctx->d_dump, ctx->P_snap, ctx->d_flush, ctx->d_Gpart, ctx->d_G, ctx->d_cqw, ctx->d_grp, ctx->d_grp_acc, ctx->d_init};
+                 ctx->d_long, ctx->d_dump, ctx->P_snap, ctx->d_flush, ctx->d_Gpart, ctx->d_G, ctx->d_cqw, ctx->d_grp, ctx->d_grp_acc, ctx->d_init, ctx->d_imu};
   for (void *p : dev)
     if (p)
       cudaFree(p);
-  void *host[] = {ctx->h_arena, ctx->h_info, ctx->h_stage, ctx->h_grp, ctx->h_init};
+  void *host[] = {ctx->h_arena, ctx->h_info, ctx->h_stage, ctx->h_grp, ctx->h_init, ctx->h_imu};
   for (void *p : host)
     if (p)
       cudaFreeHost(p);
@@ -343,6 +347,89 @@ ovb_status ovb_cov_propagate(ovb_ctx *ctx, int new_off, int p, const int *old_of
     snprintf(ctx->err, sizeof(ctx->err), "EKFPropagation: diagonal at %d is negative", ctx->h_info->neg_diag_index);
     return OVB_ERR_NEG_DIAG;
   }
+  return OVB_OK;
+}
+
+ovb_status ovb_cov_propagate_imu(ovb_ctx *ctx, int n, int steps, const double *F, const double *G, const double *qc, int new_off, const int *old_off,
+                                 const int *old_sz, int nold, int clone_off, int clone_size, const double *dnc_dt, int dt_off, double *Phi_out,
+                                 double *Q_out) {
+  if (!ctx)
+    return OVB_ERR_ARG;
+  if (n > OVB_PROP_MAX_N) {
+    snprintf(ctx->err, sizeof(ctx->err), "ovb_cov_propagate_imu: n=%d exceeds %d", n, OVB_PROP_MAX_N);
+    return OVB_ERR_CAPACITY;
+  }
+  if (n < 1 || steps < 0 || (steps > 0 && (!F || !G || !qc)) || !old_off || !old_sz || nold < 1 || new_off < 0 || new_off + n > ctx->N)
+    return OVB_ERR_ARG;
+  int q = 0;
+  for (int i = 0; i < nold; i++) {
+    if (old_off[i] < 0 || old_sz[i] < 1 || old_off[i] + old_sz[i] > ctx->N)
+      return OVB_ERR_ARG;
+    q += old_sz[i];
+  }
+  if (q != n) // Phi is n x n: its columns are the old variables
+    return OVB_ERR_ARG;
+  if (clone_size < 1 || clone_off < 0 || clone_off + clone_size > ctx->N || (dnc_dt && (dt_off < 0 || dt_off >= ctx->N || clone_size > 64)))
+    return OVB_ERR_ARG;
+  if (ctx->N + clone_size > ctx->cfg.max_state) {
+    snprintf(ctx->err, sizeof(ctx->err), "ovb_cov_propagate_imu: N+clone_size=%d exceeds max_state=%d", ctx->N + clone_size, ctx->cfg.max_state);
+    return OVB_ERR_CAPACITY;
+  }
+  const size_t nn = (size_t)n * n;
+  if (2 * nn > ctx->Hs_cap)
+    return OVB_ERR_CAPACITY;
+  OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  // staging (doubles): [F steps*nn][G steps*12n][qc steps*4][dnc_dt clone_size][old indices n ints]; Phi, Q come back in front
+  const size_t oF = 0, oG = oF + (size_t)steps * nn, oq = oG + (size_t)steps * 12 * n, od = oq + (size_t)steps * 4,
+               oi = od + (dnc_dt ? (size_t)clone_size : 0), in_doubles = oi + ((size_t)n + 1) / 2;
+  const size_t need = std::max(in_doubles, 2 * nn);
+  if (need > ctx->imu_cap) {
+    // half as much again: a run's longer gaps between frames do not regrow it each time (cudaFree waits for the whole
+    // device, other contexts' work included)
+    const size_t cap = need + need / 2;
+    cudaFree(ctx->d_imu);
+    cudaFreeHost(ctx->h_imu);
+    ctx->d_imu = nullptr, ctx->h_imu = nullptr, ctx->imu_cap = 0;
+    OVB_CUDA_CHECK(ctx, cudaMalloc(&ctx->d_imu, sizeof(double) * cap));
+    OVB_CUDA_CHECK(ctx, cudaMallocHost(&ctx->h_imu, sizeof(double) * cap));
+    ctx->imu_cap = cap;
+  }
+  double *hs = ctx->h_imu;
+  if (steps > 0) {
+    memcpy(hs + oF, F, sizeof(double) * (size_t)steps * nn);
+    memcpy(hs + oG, G, sizeof(double) * (size_t)steps * 12 * n);
+    memcpy(hs + oq, qc, sizeof(double) * (size_t)steps * 4);
+  }
+  if (dnc_dt)
+    memcpy(hs + od, dnc_dt, sizeof(double) * clone_size);
+  int *hidx = (int *)(hs + oi);
+  for (int i = 0, c = 0; i < nold; i++)
+    for (int k = 0; k < old_sz[i]; k++)
+      hidx[c++] = old_off[i] + k;
+  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->d_imu, hs, sizeof(double) * in_doubles, cudaMemcpyHostToDevice, ctx->stream));
+  // Phi and Q where ovb_cov_propagate stages them, then EKFPropagation and the clone on the same stream
+  double *Phi_dev = ctx->d_Hs, *Q_dev = ctx->d_Hs + nn;
+  if (!launch_prop_accumulate(ctx, n, steps, ctx->d_imu + oF, ctx->d_imu + oG, ctx->d_imu + oq, Phi_dev, Q_dev)) {
+    snprintf(ctx->err, sizeof(ctx->err), "ovb_cov_propagate_imu: k_prop_accumulate launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+    OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream)); // the staged inputs are in flight
+    return OVB_ERR_CUDA;
+  }
+  launch_cov_propagate(ctx, new_off, n, n, (const int *)(ctx->d_imu + oi), Phi_dev, Q_dev);
+  launch_cov_clone(ctx, clone_off, clone_size, dnc_dt ? ctx->d_imu + od : nullptr, dt_off, &ctx->d_info->neg_diag_index);
+  OVB_CUDA_CHECK(ctx, cudaGetLastError());
+  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(&ctx->h_info->neg_diag_index, &ctx->d_info->neg_diag_index, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  if (Phi_out || Q_out)
+    OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(hs, Phi_dev, sizeof(double) * 2 * nn, cudaMemcpyDeviceToHost, ctx->stream));
+  OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+  if (Phi_out)
+    memcpy(Phi_out, hs, sizeof(double) * nn);
+  if (Q_out)
+    memcpy(Q_out, hs + nn, sizeof(double) * nn);
+  if (ctx->h_info->neg_diag_index != 0x7fffffff) {
+    snprintf(ctx->err, sizeof(ctx->err), "EKFPropagation: diagonal at %d is negative", ctx->h_info->neg_diag_index);
+    return OVB_ERR_NEG_DIAG;
+  }
+  ctx->N += clone_size;
   return OVB_OK;
 }
 

@@ -9,6 +9,8 @@
 #define OVB_MAX_COLS 512          // >= 6*OVB_MAX_CLONES + 14*OVB_MAX_CAMS; also the widest H of ovb_ekf_update (config 5: n = 500)
 #define OVB_NB 16                 // TSQR panel width
 #define OVB_CR 256                // TSQR rows per chunk
+#define OVB_PROP_MAX_N 64         // widest IMU block of ovb_cov_propagate_imu (15 + IMU intrinsics is 15, 30 or 39)
+#define OVB_PROP_STEPS_RESERVE 64 // IMU steps per frame the staging of ovb_cov_propagate_imu holds from ovb_create (at n = 39)
 
 // ---- device-resident copy of the slice of State the path reads (uploaded once per update call)
 struct DevFrame {
@@ -214,6 +216,10 @@ struct ovb_ctx {
   // the counters of the last call (ovb_last_init_counters)
   DevInitSys *d_init, *h_init;
   int64_t init_counters[4];
+  // ovb_cov_propagate_imu: the per-step operands [F | G | qc | dnc_dt | old indices], one H2D copy per call; the pinned
+  // side also receives Phi and Q. Reserved at ovb_create for ordinary frames, grown with headroom beyond.
+  double *d_imu, *h_imu;
+  size_t imu_cap; // doubles
   // per-kernel profile (ovb_set_profile): CUDA events around every ovb_launch of the main stream; PDL is off while it is on
   int prof_on, prof_n;
   cudaEvent_t prof_ev[2 * 96];
@@ -274,9 +280,15 @@ void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r_max, int n
 // skip_dev (optional): the kernel returns without writing when *skip_dev is nonzero
 bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, const double *Hinv_dev, double sigma2,
                              const int *skip_dev = nullptr);
-void launch_cov_clone(ovb_ctx *ctx, int old_off, int size, const double *dnc_dt_dev, int dt_off);
+// neg_diag_dev (optional): d_info's negative-diagonal flag of a propagation enqueued before; when it is set the clone
+// leaves P alone (ovb_cov_propagate_imu then does not grow N)
+void launch_cov_clone(ovb_ctx *ctx, int old_off, int size, const double *dnc_dt_dev, int dt_off, const int *neg_diag_dev = nullptr);
 void launch_cov_marginalize(ovb_ctx *ctx, int off, int size);
 void launch_cov_propagate(ovb_ctx *ctx, int new_off, int p, int q, const int *old_idx_dev, const double *Phi_dev, const double *Q_dev);
+// Phi, Q (n x n, n <= OVB_PROP_MAX_N) accumulated over `steps` IMU steps, F [steps][n][n], G [steps][n][12], qc [steps][4];
+// false when the launch failed
+bool launch_prop_accumulate(ovb_ctx *ctx, int n, int steps, const double *F_dev, const double *G_dev, const double *qc_dev, double *Phi_dev,
+                            double *Q_dev);
 
 // ---- programmatic dependent launch (PDL) ----------------------------------------------------------------------------
 // Every kernel of the update pipeline starts with OVB_PDL_ENTER(): it lets the NEXT kernel of the stream be scheduled

@@ -1,6 +1,7 @@
 // run_simulation.cpp — rpng_sim runner (ov_msckf/src/run_simulation.cpp) on the host layer of include/ovb200_vio.hpp.
 //   ovb_run_simulation   (this file, -DOVB_SIM_ENGINE): covariance and MSCKF updates on the CUDA engine (libovb200.so)
 //   tests/cpp/run_simulation_oracle (same file, -DOVB_SIM_ORACLE, test infrastructure): the CPU oracle behind the same interface
+//   -DOVB_SIM_HOST_PROPAGATION (test infrastructure): the engine with the IMU covariance accumulation on the host
 // Usage: <exe> --traj FILE(.txt|.bin) [--cams K] [--clones C] [--msckf M] [--pts P] [--frames F] [--calib 0|1]
 //              [--est OUT.txt] [--timing [OUT.csv]] [--capture FRAME PREFIX] [--integration discrete|rk4|analytical]
 //              [--seed-init S] [--seed-perturb S] [--seed-meas S] [--runs K [--jobs J] [--out-dir DIR]]
@@ -12,6 +13,8 @@
 // line then lists every run and the mean / population standard deviation of both ATEs, the wall time and runs/s.
 #ifdef OVB_SIM_ORACLE
 #include "oracle_backend.hpp"
+#elif defined(OVB_SIM_HOST_PROPAGATION)
+#include "host_propagation_backend.hpp"
 #else
 #include "../include/ovb200_vio.hpp"
 #endif
@@ -70,7 +73,11 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
   auto backend = std::make_shared<OracleCov>();
 #else
   ovb_config cfg{0, 640, std::max(1024, o.msckf), std::max(1024, o.msckf) * 2 * (o.clones + 1) * o.cams / 2 + 1024, 0};
+#ifdef OVB_SIM_HOST_PROPAGATION
+  auto backend = std::make_shared<HostPropagationEngineCov>(cfg);
+#else
   auto backend = std::make_shared<EngineCov>(cfg);
+#endif
 #endif
   VioManager sys(vo, sp, backend);
   if (capture_frame >= 0) {
