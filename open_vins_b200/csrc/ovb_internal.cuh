@@ -271,11 +271,12 @@ bool launch_trsm_rows(ovb_ctx *ctx, double *A, int ldA, int m, int nt, const dou
 // exceeds OVB_MAX_COLS or the leading dimensions are odd
 bool launch_chol_solve_wide(ovb_ctx *ctx, double *S, int ldS, int r, double *w, double *invdiag, double *M, int ldM, int N, bool gate_only);
 void launch_reorder_R(ovb_ctx *ctx, const double *Rin, int n_all, int ldRin, double *Rout, int ldRout);
-// EKF update from an upper-trapezoidal / dense H [r x n] with column->state map in d_info (device-side sizes)
+// EKF update from an upper-trapezoidal / dense H [r x n] (r <= n) with column->state map in d_info; the residual is staged
+// in d_w. gate_only: stop after the Cholesky factor (d_w then holds w = L^-1 res, P is untouched).
 // skip_dev (optional): a device flag read after the previous kernels; nonzero marks the update failed before it starts
 // (info->not_spd), so P is left untouched and dx = 0
-void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r_max, int n_max, bool sizes_from_info, double sigma2,
-                       const double *Rdiag_dev, const int *skip_dev = nullptr);
+void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bool gate_only, double sigma2, const double *Rdiag_dev,
+                       const int *skip_dev = nullptr);
 // false: the launch was refused (shared-memory footprint) or failed; the caller must not grow N.
 // skip_dev (optional): the kernel returns without writing when *skip_dev is nonzero
 bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, const double *Hinv_dev, double sigma2,
