@@ -284,8 +284,14 @@ __device__ __forceinline__ void ct_trail_row(const CtView &sm, const double *Xk,
 // One __syncthreads per step; named barrier 1 joins the helpers after their panel rows, named barrier 2 hands block
 // column k+1 to warp 0 (it has never been seen to wait there: the helpers' first two moves are shorter than eight pivots),
 // named barrier 3 hands each factored diagonal block to the inverting warp.
-template <int THREADS>
-__device__ __forceinline__ void ct_chol_tiles(const CtView &sm, int n, int nrows, bool strict, double floor_d) {
+// Block column k (tiles (i, k), i >= k, and reciprocal pivots 8k..8k+7) is final at the barrier that ends step k. With
+// nine warps or more, warp 8 (on warp 0's sub-partition, otherwise idle) calls pub.column(sm, k) during step k + 1, so
+// that a consumer of the factor can start on it while the chain runs; the last column is the caller's to publish.
+struct CtNoPublish {
+  __device__ __forceinline__ void column(const CtView &, int) const {}
+};
+template <int THREADS, typename PUB = CtNoPublish>
+__device__ __forceinline__ void ct_chol_tiles(const CtView &sm, int n, int nrows, bool strict, double floor_d, const PUB &pub = PUB()) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   constexpr int NW = THREADS / 32, NH = NW - (NW + 3) / 4;
   static_assert(NH >= 1, "need at least one helper warp");
@@ -376,6 +382,8 @@ __device__ __forceinline__ void ct_chol_tiles(const CtView &sm, int n, int nrows
         }
       }
       CT_PROBE_T(p3);
+    } else if (wid == 8 && k > 0) {
+      pub.column(sm, k - 1);
     }
     __syncthreads();
     CT_PROBE_T(p5);

@@ -59,6 +59,34 @@ template <int N> __device__ __forceinline__ void cpa_wait() { asm volatile("cp.a
 __device__ __forceinline__ void bar_group(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 __device__ __forceinline__ int tri(int b) { return (b * (b + 1)) >> 1; }
 
+// ---- factor streaming: a factor kernel (k_cq_chol_gram of pass 1, k_cq_chol_ekf) hands its packed factor to the next
+// kernel of the stream (k_cq_solve_gram, k_cq_trsm), which PDL has made resident early, block column by block column.
+// The producer publishes on a 64-bit counter in global memory, (epoch << 6) | s:
+//   s = 1       its griddepcontrol.wait has returned: every kernel before it has completed, so the consumer may read and
+//               write its own inputs and outputs
+//   s = 2 + k   block column k of the packed factor (tiles (i, k) and reciprocal pivots 8k..8k+7) is in global memory
+// The host draws a fresh epoch for every publishing launch, so the counter only grows and is never reset. One counter
+// per context serves both producers: a producer publishes only after its griddepcontrol.wait, when the consumer of the
+// one before it has completed. The epoch is drawn on the host; an update captured into a CUDA graph would have to draw
+// it on the device instead.
+__device__ __forceinline__ void cq_pub_store(unsigned long long *ctr, unsigned long long v) {
+  asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(ctr), "l"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long cq_pub_load(const unsigned long long *ctr) {
+  unsigned long long v;
+  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(ctr) : "memory");
+  return v;
+}
+// the consumer reads the factor with the bulk-copy engine (async proxy), the producer writes it with ordinary stores
+__device__ __forceinline__ void cq_fence_proxy() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+__device__ __forceinline__ void cq_mbar_init(unsigned bar) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar) : "memory"); }
+__device__ __forceinline__ void cq_mbar_arrive(unsigned bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+// wait for phase 0 of an mbarrier; returns at once ever after (the loop stays inside the asm block: no branch for the
+// compiler to guard with convergence code in the unrolled solve)
+__device__ __forceinline__ void cq_mbar_wait(unsigned bar) {
+  asm volatile("{\n\t.reg .pred p;\n\tCQ_MWAIT:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], 0;\n\t@!p bra CQ_MWAIT;\n\t}" ::"r"(bar) : "memory");
+}
+
 // Output tile owned by warp w of Gram block blk. The Gram matrix is cut into blocks of BW x BW warp tiles (32 x 32 each);
 // only blocks bI <= bJ exist; a diagonal block keeps its upper warp tiles only. Returns false for an idle warp.
 __device__ __forceinline__ bool cq_tile_origin(int blk, int w, int BW, int nblk_side, int &ci, int &cj, int &offI, int &offJ, bool &diag) {
@@ -313,9 +341,47 @@ struct CqCholSmem {
 
 namespace {
 
+// Publication of the packed factor of an n-column factorisation (ctr == nullptr: nobody streams). column() is
+// ct_chol_tiles' hook (warp 8); it stores tiles (i, k) and pivots 8k..8k+7 at the addresses and with the values the
+// epilogue's copy writes, then the count. Each lane's stores, a fence, then one lane's release of the count.
+struct CqPublish {
+  double *Lpk;
+  unsigned long long *ctr, epoch;
+  int n;
+  __device__ __forceinline__ void column(const CtView &sm, int k) const {
+    if (ctr == nullptr)
+      return;
+    const int lane = threadIdx.x & 31, NB = (n + 7) >> 3;
+    for (int i = k; i < NB; i++) {
+      const size_t o = (size_t)(ct_tri(i) + k) * 64 + 2 * lane;
+      *reinterpret_cast<double2 *>(Lpk + o) = *reinterpret_cast<const double2 *>(sm.T + o);
+    }
+    if (lane < 8)
+      Lpk[CQ_PK_INV + 8 * k + lane] = (8 * k + lane < n) ? sm.invd[8 * k + lane] : 1.0;
+    cq_fence_proxy();
+    __threadfence();
+    __syncwarp();
+    if (lane == 0)
+      cq_pub_store(ctr, (epoch << 6) | (unsigned long long)(k + 2));
+  }
+  // the epilogue's copy starts past what column() has published: the last block column (its diagonal tile) and the pivots
+  __device__ __forceinline__ int first_tile_el() const { return ctr ? (tri((n + 7) >> 3) - 1) * 64 : 0; }
+  __device__ __forceinline__ int first_pivot() const { return ctr ? 8 * (((n + 7) >> 3) - 1) : 0; }
+  // the whole CTA, after its share of the epilogue's copy: the last column's count
+  __device__ __forceinline__ void finish() const {
+    if (ctr == nullptr)
+      return;
+    cq_fence_proxy();
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0)
+      cq_pub_store(ctr, (epoch << 6) | (unsigned long long)(((n + 7) >> 3) + 1));
+  }
+};
+
 // The factorisation proper lives in chol_tiles.cuh (shared with the per-feature gate); this kernel family runs it with
 // CQ_CHOL_T threads (256 / 512 / 640 were measured: 40.9 / 37.7 / 38.9 us against 36.8 us at 384, n = 155).
-__device__ __forceinline__ void cq_chol_tiles(CqCholSmem &sm, int n, int nrows, bool strict, double floor_d) {
+__device__ __forceinline__ void cq_chol_tiles(CqCholSmem &sm, int n, int nrows, bool strict, double floor_d, const CqPublish &pub) {
   CtView v;
   v.T = sm.T;
   v.Xp0 = sm.Xp[0];
@@ -326,7 +392,7 @@ __device__ __forceinline__ void cq_chol_tiles(CqCholSmem &sm, int n, int nrows, 
   v.dummyT = sm.dummyT;
   v.dummyX = sm.dummyX;
   v.flag = &sm.flag;
-  ct_chol_tiles<CQ_CHOL_T>(v, n, nrows, strict, floor_d);
+  ct_chol_tiles<CQ_CHOL_T>(v, n, nrows, strict, floor_d, pub);
 }
 
 // stage the lower triangle of a row-major global matrix (rows < nrows, cols < n; rows >= n come from `rhs` when given)
@@ -363,8 +429,13 @@ __device__ __forceinline__ double cq_el(const double *T, int i, int j) { return 
 } // namespace
 
 // Gram mode: L L' = G + shift_rel * max(diag G) * I; writes L (= R') in the packed layout above to Lpk. ldG even.
-__global__ void __launch_bounds__(CQ_CHOL_T) k_cq_chol_gram(const double *__restrict__ G, int ldG, int n, double shift_rel, double *__restrict__ Lpk, int tiled) {
+// pub_ctr != nullptr: streams L to the next kernel on that counter (see cq_pub_store).
+__global__ void __launch_bounds__(CQ_CHOL_T) k_cq_chol_gram(const double *__restrict__ G, int ldG, int n, double shift_rel, double *__restrict__ Lpk, int tiled,
+                                                           unsigned long long *pub_ctr, unsigned long long epoch) {
   OVB_PDL_ENTER();
+  if (pub_ctr != nullptr && threadIdx.x == 0)
+    cq_pub_store(pub_ctr, (epoch << 6) | 1ull);
+  const CqPublish pub{Lpk, pub_ctr, epoch, n};
   extern __shared__ __align__(16) unsigned char cq_raw[];
   CqCholSmem &sm = *reinterpret_cast<CqCholSmem *>(cq_raw);
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -434,15 +505,16 @@ __global__ void __launch_bounds__(CQ_CHOL_T) k_cq_chol_gram(const double *__rest
 #ifdef CQ_PROBE
   const long long q1 = clock64();
 #endif
-  cq_chol_tiles(sm, n, n, false, 0.25 * shift);
+  cq_chol_tiles(sm, n, n, false, 0.25 * shift, pub);
 #ifdef CQ_PROBE
   const long long q2 = clock64();
 #endif
   const int NB = (n + 7) >> 3;
-  for (int e = 2 * tid; e < tri(NB) * 64; e += 2 * CQ_CHOL_T)
+  for (int e = pub.first_tile_el() + 2 * tid; e < tri(NB) * 64; e += 2 * CQ_CHOL_T)
     *reinterpret_cast<double2 *>(Lpk + e) = *reinterpret_cast<const double2 *>(sm.T + e);
-  for (int e = tid; e < CQ_MAXB * 8; e += CQ_CHOL_T)
+  for (int e = pub.first_pivot() + tid; e < CQ_MAXB * 8; e += CQ_CHOL_T)
     Lpk[CQ_PK_INV + e] = (e < n) ? sm.invd[e] : 1.0;
+  pub.finish();
 #ifdef CQ_PROBE
   if (tid == 0)
     printf("chol_gram n=%d: load %lld factor %lld store %lld cycles\n", n, q1 - q0, q2 - q1, clock64() - q2);
@@ -453,11 +525,15 @@ __global__ void __launch_bounds__(CQ_CHOL_T) k_cq_chol_gram(const double *__rest
 // factorisation of wide systems: S (r x r, lower triangle in global memory), optionally with the residual as one right-hand-
 // side row (res != nullptr) -> L written back over the lower triangle of S, w = L^-1 res, 1/diag(L), the packed factor for
 // k_cq_trsm. floor_dev == nullptr: strict, a non-positive pivot raises info->not_spd; else pivots are floored at *floor_dev
-// (shifted Gram matrices). ldS even.
+// (shifted Gram matrices). ldS even. pub_ctr != nullptr (requires Lpk): streams the packed factor to the next kernel on
+// that counter (see cq_pub_store), ahead of the other outputs.
 __global__ void __launch_bounds__(CQ_CHOL_T) k_cq_chol_ekf(double *__restrict__ S, int ldS, int r, const double *__restrict__ res, double *__restrict__ w,
                                                           double *__restrict__ invdiag, DevUpdateInfo *__restrict__ info, double *__restrict__ Lpk,
-                                                          const double *__restrict__ floor_dev) {
+                                                          const double *__restrict__ floor_dev, unsigned long long *pub_ctr, unsigned long long epoch) {
   OVB_PDL_ENTER();
+  if (pub_ctr != nullptr && threadIdx.x == 0)
+    cq_pub_store(pub_ctr, (epoch << 6) | 1ull);
+  const CqPublish pub{Lpk, pub_ctr, epoch, r};
   extern __shared__ __align__(16) unsigned char cq_raw[];
   CqCholSmem &sm = *reinterpret_cast<CqCholSmem *>(cq_raw);
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -465,9 +541,17 @@ __global__ void __launch_bounds__(CQ_CHOL_T) k_cq_chol_ekf(double *__restrict__ 
   cq_load_tiles(sm, S, (size_t)ldS, r, nrows, res, 0);
   __syncthreads();
   if (floor_dev != nullptr)
-    cq_chol_tiles(sm, r, nrows, false, *floor_dev);
+    cq_chol_tiles(sm, r, nrows, false, *floor_dev, pub);
   else
-    cq_chol_tiles(sm, r, nrows, true, 0.0);
+    cq_chol_tiles(sm, r, nrows, true, 0.0, pub);
+  if (Lpk != nullptr) { // the factor as k_cq_trsm consumes it (Y = M L^-T)
+    const int NB = (r + 7) >> 3;
+    for (int e = pub.first_tile_el() + 2 * tid; e < tri(NB) * 64; e += 2 * CQ_CHOL_T)
+      *reinterpret_cast<double2 *>(Lpk + e) = *reinterpret_cast<const double2 *>(sm.T + e);
+    for (int e = pub.first_pivot() + tid; e < CQ_MAXB * 8; e += CQ_CHOL_T)
+      Lpk[CQ_PK_INV + e] = (e < r) ? sm.invd[e] : 1.0;
+    pub.finish();
+  }
   for (int i = wid; i < r; i += CQ_CHOL_T / 32)
     for (int j = lane; j <= i; j += 32)
       S[(size_t)i * ldS + j] = cq_el(sm.T, i, j);
@@ -477,13 +561,6 @@ __global__ void __launch_bounds__(CQ_CHOL_T) k_cq_chol_ekf(double *__restrict__ 
   if (invdiag != nullptr)
     for (int j = tid; j < r; j += CQ_CHOL_T)
       invdiag[j] = sm.invd[j];
-  if (Lpk != nullptr) { // the factor as k_cq_trsm consumes it (Y = M L^-T)
-    const int NB = (r + 7) >> 3;
-    for (int e = 2 * tid; e < tri(NB) * 64; e += 2 * CQ_CHOL_T)
-      *reinterpret_cast<double2 *>(Lpk + e) = *reinterpret_cast<const double2 *>(sm.T + e);
-    for (int e = tid; e < CQ_MAXB * 8; e += CQ_CHOL_T)
-      Lpk[CQ_PK_INV + e] = (e < r) ? sm.invd[e] : 1.0;
-  }
   if (tid == 0 && sm.flag && info != nullptr)
     info->not_spd = 1;
 }
@@ -505,12 +582,16 @@ __global__ void __launch_bounds__(CQ_CHOL_T) k_cq_chol_ekf(double *__restrict__ 
 #define CQ_TRSM_SMEM (sizeof(double) * ((size_t)CQ_PK_DOUBLES + (size_t)(CQ_TRSM_T / 32) * CQ_TRSM_NH * 2 * 32))
 // All control flow around the DMMAs is compile-time (NH blocks, padded with zero tiles): a run-time bound inside the
 // unrolled loops makes the compiler guard every mma.sync / shfl.sync with convergence code and several code versions.
-template <int NH>
-__device__ __forceinline__ void cq_trsm_half(double (&acc)[NH][2], int b0, const double *Lt, const double *Ri, double *xs, int lane) {
+// WAIT: the factor is streaming in (cq_stream_fetch); block B reads block column B only, so it waits for mbarrier
+// cbar + 8B first.
+template <int NH, bool WAIT = false>
+__device__ __forceinline__ void cq_trsm_half(double (&acc)[NH][2], int b0, const double *Lt, const double *Ri, double *xs, int lane, unsigned cbar = 0) {
   const int g = lane >> 2, q = lane & 3;
 #pragma unroll
   for (int jb = 0; jb < NH; jb++) {
     const int B = b0 + jb;
+    if constexpr (WAIT)
+      cq_mbar_wait(cbar + 8 * B);
     const double *Ld = Lt + (size_t)(tri(B) + B) * 64; // R[8B+t][8B+c] = Ld[c*8 + t], t <= c
     const double *ri = Ri + B * 8;
     double x[8];
@@ -606,21 +687,106 @@ __device__ __forceinline__ void cq_fetch_factor(double *Lt, double *Ri, const do
   __syncthreads();
 }
 
-// NH1 + NH2 >= ceil(nt / 8); NH2 == 0: single half
-template <int NH1, int NH2>
-__global__ void __launch_bounds__(CQ_TRSM_T) k_cq_trsm(double *__restrict__ A, int ldA, int m, int nt, const double *__restrict__ Lpk) {
-  OVB_PDL_ENTER();
+// Consumer side of the factor streaming (see cq_pub_store). bars: NBP + 1 mbarriers in shared memory. bars[0] completes
+// once the producer has passed its griddepcontrol.wait (from then on the consumer may touch its inputs and outputs),
+// bars[1 + j] once block column j of the factor is in Lt / Ri, at the positions cq_fetch_factor fills. Ends with a
+// barrier of all NT threads.
+template <int NBP, int NT>
+__device__ __forceinline__ void cq_stream_init(unsigned long long *bars, double *Lt, double *Ri, int NB) {
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    for (int j = 0; j <= NBP; j++)
+      cq_mbar_init(s_u32(bars + j));
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  for (int e = tri(NB) * 64 + tid; e < tri(NBP) * 64; e += NT)
+    Lt[e] = 0.0;
+  for (int e = NB * 8 + tid; e < NBP * 8; e += NT)
+    Ri[e] = 1.0;
+  __syncthreads();
+}
+
+// How long the consumer polls before it stops (ns): far beyond a factorisation (tens of us); a time-sliced GPU may
+// still get there, so the consumer then waits for the producer grid to complete and takes the rest of the factor at once.
+#define CQ_STREAM_POLL_NS 20000000ull
+
+// One thread of a warp that does nothing else: polls the counter (backing off with __nanosleep) and bulk-copies each
+// block column of the factor as it is published; the padding columns NB..NBP-1 (cq_stream_init) complete at once.
+// Returns once every copy has landed and the producer grid has completed (griddepcontrol.wait): a consumer never
+// completes before its producer, so the kernels after it see the producer's other outputs in plain stream order.
+__device__ void cq_stream_fetch(unsigned long long *bars, double *Lt, double *Ri, const double *__restrict__ Lpk, int NB, int NBP,
+                                const unsigned long long *ctr, unsigned long long epoch) {
+  const unsigned long long base = epoch << 6;
+  unsigned long long t0, t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+  bool poll = true;
+  auto reach = [&](int s) {
+    while (poll && cq_pub_load(ctr) < (base | (unsigned long long)s)) {
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+      if (t - t0 > CQ_STREAM_POLL_NS) {
+        asm volatile("griddepcontrol.wait;" ::: "memory");
+        poll = false;
+      } else {
+        __nanosleep(64);
+      }
+    }
+  };
+  reach(1);
+  cq_mbar_arrive(s_u32(bars));
+  for (int j = NB; j < NBP; j++)
+    cq_mbar_arrive(s_u32(bars + 1 + j));
+  for (int j = 0; j < NB; j++) {
+    reach(j + 2);
+    cq_fence_proxy();
+    const unsigned bar = s_u32(bars + 1 + j);
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((unsigned)((NB - j) * 64 + 8) * 8u) : "memory");
+    for (int i = j; i < NB; i++) {
+      const size_t o = (size_t)(tri(i) + j) * 64;
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], 512, [%2];" ::"r"(s_u32(Lt + o)), "l"(Lpk + o), "r"(bar)
+                   : "memory");
+    }
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], 64, [%2];" ::"r"(s_u32(Ri + 8 * j)), "l"(Lpk + CQ_PK_INV + 8 * j),
+                 "r"(bar)
+                 : "memory");
+  }
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  for (int j = 0; j < NB; j++)
+    cq_mbar_wait(s_u32(bars + 1 + j));
+}
+
+// NH1 + NH2 >= ceil(nt / 8); NH2 == 0: single half. STREAM: the factor streams in from the k_cq_chol_ekf launched just
+// before on (pub_ctr, epoch), fetched by the last warp (a 21st warp would cut the registers per thread from 96 to 80);
+// the other warps take the row groups and read their rows once that producer has passed its own wait.
+template <int NH1, int NH2, bool STREAM>
+__device__ __forceinline__ void cq_trsm_rows(double *__restrict__ A, int ldA, int m, int nt, const double *__restrict__ Lpk,
+                                             const unsigned long long *__restrict__ pub_ctr, unsigned long long epoch) {
   extern __shared__ __align__(16) double tsm[];
   double *Lt = tsm;
   double *Ri = tsm + CQ_PK_INV;
   double *Xs = tsm + CQ_PK_DOUBLES; // per warp: first-half A-operand fragments [NH1][2][32]
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, g = lane >> 2, q = lane & 3;
-  cq_fetch_factor<NH1 + NH2, CQ_TRSM_T>(Lt, Ri, Lpk, (nt + 7) >> 3);
+  unsigned cbar = 0;
+  if constexpr (STREAM) {
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    __shared__ __align__(8) unsigned long long bars[CQ_MAXB + 1];
+    cq_stream_init<NH1 + NH2, CQ_TRSM_T>(bars, Lt, Ri, (nt + 7) >> 3);
+    if (wid == CQ_TRSM_T / 32 - 1) {
+      if (lane == 0)
+        cq_stream_fetch(bars, Lt, Ri, Lpk, (nt + 7) >> 3, NH1 + NH2, pub_ctr, epoch);
+      return;
+    }
+    cq_mbar_wait(s_u32(bars));
+    cbar = s_u32(bars + 1);
+  } else {
+    OVB_PDL_ENTER();
+    cq_fetch_factor<NH1 + NH2, CQ_TRSM_T>(Lt, Ri, Lpk, (nt + 7) >> 3);
+  }
   double *xs = Xs + (size_t)wid * (CQ_TRSM_NH * 2 * 32);
   const int ngroups = (m + 7) >> 3;
   // row groups are dealt round-robin over the CTAs first (warp w of CTA b takes group b + w * gridDim.x): a short matrix puts
   // one group on each SM instead of twenty on the first
-  for (int rg = blockIdx.x + gridDim.x * wid; rg < ngroups; rg += gridDim.x * (CQ_TRSM_T / 32)) {
+  constexpr int NSW = CQ_TRSM_T / 32 - (STREAM ? 1 : 0); // solving warps
+  for (int rg = blockIdx.x + gridDim.x * wid; rg < ngroups; rg += gridDim.x * NSW) {
     const int row = 8 * rg + g;
     const bool row_ok = row < m;
     double *arow = A + (size_t)row * ldA;
@@ -633,7 +799,7 @@ __global__ void __launch_bounds__(CQ_TRSM_T) k_cq_trsm(double *__restrict__ A, i
 #ifdef CQ_PROBE
       t1 = clock64();
 #endif
-      cq_trsm_half<NH1>(acc, 0, Lt, Ri, NH2 > 0 ? xs : nullptr, lane);
+      cq_trsm_half<NH1, STREAM>(acc, 0, Lt, Ri, NH2 > 0 ? xs : nullptr, lane, cbar);
 #ifdef CQ_PROBE
       t2 = clock64();
 #endif
@@ -657,7 +823,7 @@ __global__ void __launch_bounds__(CQ_TRSM_T) k_cq_trsm(double *__restrict__ A, i
 #ifdef CQ_PROBE
       t3 = clock64();
 #endif
-      cq_trsm_half<NH2>(acc, NH1, Lt, Ri, nullptr, lane);
+      cq_trsm_half<NH2, STREAM>(acc, NH1, Lt, Ri, nullptr, lane, cbar);
 #ifdef CQ_PROBE
       t4 = clock64();
 #endif
@@ -670,18 +836,47 @@ __global__ void __launch_bounds__(CQ_TRSM_T) k_cq_trsm(double *__restrict__ A, i
 #endif
   }
 }
+// two overloads of one kernel name: the streaming one takes the counter
+template <int NH1, int NH2>
+__global__ void __launch_bounds__(CQ_TRSM_T) k_cq_trsm(double *__restrict__ A, int ldA, int m, int nt, const double *__restrict__ Lpk) {
+  cq_trsm_rows<NH1, NH2, false>(A, ldA, m, nt, Lpk, nullptr, 0);
+}
+template <int NH1, int NH2>
+__global__ void __launch_bounds__(CQ_TRSM_T) k_cq_trsm(double *__restrict__ A, int ldA, int m, int nt, const double *__restrict__ Lpk,
+                                                      const unsigned long long *__restrict__ pub_ctr, unsigned long long epoch) {
+  cq_trsm_rows<NH1, NH2, true>(A, ldA, m, nt, Lpk, pub_ctr, epoch);
+}
+using CqTrsmKernel = void (*)(double *, int, int, int, const double *);
+using CqTrsmStreamKernel = void (*)(double *, int, int, int, const double *, const unsigned long long *, unsigned long long);
 
-static void cq_launch_trsm(ovb_ctx *ctx, int ctas, double *A, int ldA, int m, int nt, const double *Lpk) {
+template <bool STREAM>
+static void cq_launch_trsm_t(ovb_ctx *ctx, int ctas, double *A, int ldA, int m, int nt, const double *Lpk, const unsigned long long *pub_ctr,
+                             unsigned long long epoch) {
   const int NB = (nt + 7) / 8;
   const size_t smem = CQ_TRSM_SMEM;
+  const dim3 grid(ctas), block(CQ_TRSM_T);
+  auto go = [&](auto plain, auto streaming) {
+    if constexpr (STREAM)
+      ovb_launch(ctx, streaming, grid, block, smem, A, ldA, m, nt, Lpk, pub_ctr, epoch);
+    else
+      ovb_launch(ctx, plain, grid, block, smem, A, ldA, m, nt, Lpk);
+  };
   if (NB <= 5)
-    ovb_launch(ctx, k_cq_trsm<5, 0>, dim3(ctas), dim3(CQ_TRSM_T), smem, A, ldA, m, nt, Lpk);
+    go((CqTrsmKernel)k_cq_trsm<5, 0>, (CqTrsmStreamKernel)k_cq_trsm<5, 0>);
   else if (NB <= 10)
-    ovb_launch(ctx, k_cq_trsm<10, 0>, dim3(ctas), dim3(CQ_TRSM_T), smem, A, ldA, m, nt, Lpk);
+    go((CqTrsmKernel)k_cq_trsm<10, 0>, (CqTrsmStreamKernel)k_cq_trsm<10, 0>);
   else if (NB <= 15)
-    ovb_launch(ctx, k_cq_trsm<10, 5>, dim3(ctas), dim3(CQ_TRSM_T), smem, A, ldA, m, nt, Lpk);
+    go((CqTrsmKernel)k_cq_trsm<10, 5>, (CqTrsmStreamKernel)k_cq_trsm<10, 5>);
   else
-    ovb_launch(ctx, k_cq_trsm<10, 10>, dim3(ctas), dim3(CQ_TRSM_T), smem, A, ldA, m, nt, Lpk);
+    go((CqTrsmKernel)k_cq_trsm<10, 10>, (CqTrsmStreamKernel)k_cq_trsm<10, 10>);
+}
+// pub_ctr != nullptr: the factor streams in from the factor kernel launched just before on (pub_ctr, epoch)
+static void cq_launch_trsm(ovb_ctx *ctx, int ctas, double *A, int ldA, int m, int nt, const double *Lpk, const unsigned long long *pub_ctr = nullptr,
+                           unsigned long long epoch = 0) {
+  if (pub_ctr != nullptr)
+    cq_launch_trsm_t<true>(ctx, ctas, A, ldA, m, nt, Lpk, pub_ctr, epoch);
+  else
+    cq_launch_trsm_t<false>(ctx, ctas, A, ldA, m, nt, Lpk, pub_ctr, epoch);
 }
 
 // ------------------------------------------------------------------------------------------------------------ pass 2: solve + Gram
@@ -711,14 +906,16 @@ __host__ __device__ __forceinline__ int cq_sg_pitch(int BW, int NBP) {
 // one warp's 8-row group solved in place: xrow = the lane's row (8*NBP columns, zero past nt), k_cq_trsm's row solve; the
 // second half takes its A-operands from the solved first half in the row. Lanes with !row_ok (past the rows to solve)
 // load zeros and store nothing; their xrow must still be a row of the warp's group.
+// The factor may still be streaming in: block B of the solve waits for mbarrier cbar + 8B (the second half's leading
+// product reads block columns < NH1 only, which the first half has waited for).
 template <int NH1, int NH2>
-__device__ __forceinline__ void cq_solve_group(double *xrow, bool row_ok, const double *Lt, const double *Ri, int lane) {
+__device__ __forceinline__ void cq_solve_group(double *xrow, bool row_ok, const double *Lt, const double *Ri, int lane, unsigned cbar) {
   constexpr int NBP = NH1 + NH2;
   const int g = lane >> 2, q = lane & 3;
   {
     double acc[NH1][2];
     cq_trsm_load<NH1>(acc, xrow, row_ok, 0, 8 * NBP, q);
-    cq_trsm_half<NH1>(acc, 0, Lt, Ri, nullptr, lane);
+    cq_trsm_half<NH1, true>(acc, 0, Lt, Ri, nullptr, lane, cbar);
     cq_trsm_store<NH1>(acc, xrow, row_ok, 0, 8 * NBP, q);
   }
   if constexpr (NH2 > 0) {
@@ -736,15 +933,21 @@ __device__ __forceinline__ void cq_solve_group(double *xrow, bool row_ok, const 
         dmma(acc[j][0], acc[j][1], af1, lf[4]);
       }
     }
-    cq_trsm_half<NH2>(acc, NH1, Lt, Ri, nullptr, lane);
+    cq_trsm_half<NH2, true>(acc, NH1, Lt, Ri, nullptr, lane, cbar);
     cq_trsm_store<NH2>(acc, xrow, row_ok, NH1, 8 * NBP, q);
   }
 }
 
+// R1 streams in from pass 1's k_cq_chol_gram on (pub_ctr, epoch): the first round's rows are issued as soon as that
+// kernel has passed its own wait, so they load while the pivot chain runs, and each row group's solve follows the
+// factor block column by block column. Warp 15 fetches the factor (cq_stream_fetch; a 17th warp would cut the registers
+// per thread from 128 to 96) and only then joins the first round: it solves its row group there, if the round has
+// one, after the last block column has come in. The Gram tiles take warps 0..14 at most.
 template <int NH1, int NH2>
 __global__ void __launch_bounds__(CQ_GRAM_T) k_cq_solve_gram(const double *__restrict__ A, int ldA, int m, int nt, const double *__restrict__ Lpk, int slab_rows,
-                                                            int cb, int ntail_max, int BW, double *__restrict__ Gpart, double *__restrict__ Qtail) {
-  OVB_PDL_ENTER();
+                                                          int cb, int ntail_max, int BW, double *__restrict__ Gpart, double *__restrict__ Qtail,
+                                                          const unsigned long long *__restrict__ pub_ctr, unsigned long long epoch) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   extern __shared__ __align__(16) double ssm[];
   double *Lt = ssm;
   double *Ri = ssm + CQ_PK_INV;
@@ -757,29 +960,49 @@ __global__ void __launch_bounds__(CQ_GRAM_T) k_cq_solve_gram(const double *__res
   auto split_at = [&](int rc) { return r1 - rc > cb && r1 - rc <= 8 * (CQ_GRAM_T / 32); };
   // rows the buffer takes in the round at rc (a partial k-step is padded with zero rows)
   auto nbuf_at = [&](int rc) { return split_at(rc) ? cb & ~7 : min(cb, (r1 - rc + 3) & ~3); };
-  // the first round's rows are in flight while the factor arrives
-  if (r0 < r1)
-    cq_issue_rows<CQ_GRAM_T>(X, pitch, A, ldA, r0, nbuf_at(r0), r1, nt, 0, 0, pitch - 4, 1);
-  cq_fetch_factor<NBP, CQ_GRAM_T>(Lt, Ri, Lpk, (nt + 7) >> 3);
+  constexpr int NF = CQ_GRAM_T - 32; // threads other than the fetching warp
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, g = lane >> 2, q = lane & 3, lr = 8 * wid + g;
+  const bool fetcher = threadIdx.x >= NF;
+  __shared__ __align__(8) unsigned long long bars[CQ_MAXB + 1];
+  cq_stream_init<NBP, CQ_GRAM_T>(bars, Lt, Ri, (nt + 7) >> 3);
+  const unsigned cbar = s_u32(bars + 1);
+  if (fetcher) {
+    if (lane == 0)
+      cq_stream_fetch(bars, Lt, Ri, Lpk, (nt + 7) >> 3, NBP, pub_ctr, epoch);
+    __syncwarp();
+  } else {
+    cq_mbar_wait(s_u32(bars)); // A may be read, Gpart and the scratch written (pass 1's k_cq_reduce has completed)
+    // the first round's rows are in flight while the factor arrives
+    if (r0 < r1)
+      cq_issue_rows<NF>(X, pitch, A, ldA, r0, nbuf_at(r0), r1, nt, 0, 0, pitch - 4, 1);
+  }
   for (int rc = r0, nbuf = nbuf_at(r0), ntail = 0; rc < r1; rc += nbuf + ntail, nbuf = nbuf_at(rc)) {
     ntail = split_at(rc) ? (r1 - rc - nbuf + 3) & ~3 : 0;
     const int nact = nbuf + ntail;
-    if (rc > r0)
+    const bool first = rc == r0;
+    if (!first)
       cq_issue_rows<CQ_GRAM_T>(X, pitch, A, ldA, rc, nbuf, r1, nt, 0, 0, pitch - 4, 1);
     // the rows past the buffer into the scratch, zero-padded like the buffer (the solve then reads every row alike)
-    for (int e = threadIdx.x; e < ntail * (pitch - 4); e += CQ_GRAM_T) {
-      const int k = e / (pitch - 4), col = e - k * (pitch - 4), r = rc + nbuf + k;
-      tail[(size_t)k * pitch + col] = (r < r1 && col < nt) ? A[(size_t)r * ldA + col] : 0.0;
-    }
+    if (!(first && fetcher))
+      for (int e = threadIdx.x; e < ntail * (pitch - 4); e += first ? NF : CQ_GRAM_T) {
+        const int k = e / (pitch - 4), col = e - k * (pitch - 4), r = rc + nbuf + k;
+        tail[(size_t)k * pitch + col] = (r < r1 && col < nt) ? A[(size_t)r * ldA + col] : 0.0;
+      }
     cpa_wait<0>();
-    __syncthreads();
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, g = lane >> 2, q = lane & 3, lr = 8 * wid + g;
+    if (!first) {
+      bar_group(1, CQ_GRAM_T);
+    } else if (fetcher) { // the rows the others staged (named barrier 3), once the whole factor is in
+      asm volatile("bar.sync 3, %0;" ::"n"(CQ_GRAM_T) : "memory");
+    } else {
+      asm volatile("bar.arrive 3, %0;" ::"n"(CQ_GRAM_T) : "memory");
+      bar_group(2, NF);
+    }
     // a row group is all in the buffer or all in the scratch
     if (8 * wid < nbuf)
-      cq_solve_group<NH1, NH2>(X + (size_t)min(lr, nbuf - 1) * pitch, lr < nbuf, Lt, Ri, lane);
+      cq_solve_group<NH1, NH2>(X + (size_t)min(lr, nbuf - 1) * pitch, lr < nbuf, Lt, Ri, lane, cbar);
     else if (8 * wid < nact)
-      cq_solve_group<NH1, NH2>(tail + (size_t)min(lr - nbuf, ntail - 1) * pitch, lr < nact, Lt, Ri, lane);
-    __syncthreads();
+      cq_solve_group<NH1, NH2>(tail + (size_t)min(lr - nbuf, ntail - 1) * pitch, lr < nact, Lt, Ri, lane, cbar);
+    bar_group(1, CQ_GRAM_T);
     int ci, cj, offI, offJ;
     bool diag;
     const bool active = cq_tile_origin(0, wid, BW, 1, ci, cj, offI, offJ, diag);
@@ -804,7 +1027,7 @@ __global__ void __launch_bounds__(CQ_GRAM_T) k_cq_solve_gram(const double *__res
         for (int b = 0; b < 4; b++)
           *reinterpret_cast<double2 *>(part + a * 256 + 8 * b) = make_double2(acc[a][b][0], acc[a][b][1]);
     }
-    __syncthreads();
+    bar_group(1, CQ_GRAM_T);
   }
 }
 
@@ -831,24 +1054,24 @@ static size_t cq_solve_gram_scratch(int nslab, int nt, int BW, int slab_rows) {
 
 template <int NH1, int NH2>
 static void cq_launch_solve_gram_t(ovb_ctx *ctx, int nslab, const double *A, int ldA, int m, int nt, const double *Lpk, int slab_rows, int BW, double *Gpart,
-                                   double *Qtail) {
+                                   double *Qtail, const unsigned long long *pub_ctr, unsigned long long epoch) {
   const CqSgShape s = cq_sg_shape(nt, BW, slab_rows);
   const size_t smem = sizeof(double) * (CQ_PK_DOUBLES + (size_t)s.cb * s.pitch);
-  ovb_launch(ctx, k_cq_solve_gram<NH1, NH2>, dim3(nslab), dim3(CQ_GRAM_T), smem, A, ldA, m, nt, Lpk, slab_rows, s.cb, s.ntail, BW, Gpart, Qtail);
+  ovb_launch(ctx, k_cq_solve_gram<NH1, NH2>, dim3(nslab), dim3(CQ_GRAM_T), smem, A, ldA, m, nt, Lpk, slab_rows, s.cb, s.ntail, BW, Gpart, Qtail, pub_ctr, epoch);
 }
 // slabs of slab_rows rows (a multiple of 4), BW = ceil(nt / 32): the Gram geometry of the narrow path; Qtail: scratch of
-// cq_solve_gram_scratch() doubles
+// cq_solve_gram_scratch() doubles; Lpk streams in from the k_cq_chol_gram launched just before on (pub_ctr, epoch)
 static void cq_launch_solve_gram(ovb_ctx *ctx, int nslab, const double *A, int ldA, int m, int nt, const double *Lpk, int slab_rows, int BW, double *Gpart,
-                                 double *Qtail) {
+                                 double *Qtail, const unsigned long long *pub_ctr, unsigned long long epoch) {
   const int NB = (nt + 7) / 8;
   if (NB <= 5)
-    cq_launch_solve_gram_t<5, 0>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail);
+    cq_launch_solve_gram_t<5, 0>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail, pub_ctr, epoch);
   else if (NB <= 10)
-    cq_launch_solve_gram_t<10, 0>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail);
+    cq_launch_solve_gram_t<10, 0>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail, pub_ctr, epoch);
   else if (NB <= 15)
-    cq_launch_solve_gram_t<10, 5>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail);
+    cq_launch_solve_gram_t<10, 5>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail, pub_ctr, epoch);
   else
-    cq_launch_solve_gram_t<10, 10>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail);
+    cq_launch_solve_gram_t<10, 10>(ctx, nslab, A, ldA, m, nt, Lpk, slab_rows, BW, Gpart, Qtail, pub_ctr, epoch);
 }
 
 // ------------------------------------------------------------------------------------------------------------ R = R2 R1
@@ -1071,10 +1294,14 @@ static bool cq_attrs(ovb_ctx *ctx) {
     cudaFuncSetAttribute(k_cq_gram, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
     cudaFuncSetAttribute(k_cq_chol_gram, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CqCholSmem));
     cudaFuncSetAttribute(k_cq_chol_ekf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CqCholSmem));
-    cudaFuncSetAttribute(k_cq_trsm<5, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
-    cudaFuncSetAttribute(k_cq_trsm<10, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
-    cudaFuncSetAttribute(k_cq_trsm<10, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
-    cudaFuncSetAttribute(k_cq_trsm<10, 10>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
+    cudaFuncSetAttribute((CqTrsmKernel)k_cq_trsm<5, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
+    cudaFuncSetAttribute((CqTrsmStreamKernel)k_cq_trsm<5, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
+    cudaFuncSetAttribute((CqTrsmKernel)k_cq_trsm<10, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
+    cudaFuncSetAttribute((CqTrsmStreamKernel)k_cq_trsm<10, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
+    cudaFuncSetAttribute((CqTrsmKernel)k_cq_trsm<10, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
+    cudaFuncSetAttribute((CqTrsmStreamKernel)k_cq_trsm<10, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
+    cudaFuncSetAttribute((CqTrsmKernel)k_cq_trsm<10, 10>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
+    cudaFuncSetAttribute((CqTrsmStreamKernel)k_cq_trsm<10, 10>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CQ_TRSM_SMEM);
     cudaFuncSetAttribute(k_cq_solve_gram<5, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, CQ_SG_SMEM);
     cudaFuncSetAttribute(k_cq_solve_gram<10, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, CQ_SG_SMEM);
     cudaFuncSetAttribute(k_cq_solve_gram<10, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, CQ_SG_SMEM);
@@ -1103,9 +1330,14 @@ static bool cq_ensure_G(ovb_ctx *ctx) {
 
 // EKF Cholesky through the DMMA kernel when S (+ the residual row) fits its tile store. With one right-hand-side row the
 // last row block may spill past CQ_MAXB blocks; the packed factor (for the register solve) is only offered when it fits.
-bool launch_chol_ekf_dmma(ovb_ctx *ctx, double *S, int ldS, int r, const double *res, double *w, double *invdiag, double **Lpk_out) {
+// epoch_out != nullptr: the packed factor is streamed to the launch_trsm_rows that follows, on the epoch written there
+// (0: not streamed).
+bool launch_chol_ekf_dmma(ovb_ctx *ctx, double *S, int ldS, int r, const double *res, double *w, double *invdiag, double **Lpk_out,
+                          unsigned long long *epoch_out) {
   if (Lpk_out)
     *Lpk_out = nullptr;
+  if (epoch_out)
+    *epoch_out = 0;
   if (r + 1 > CQ_MAXRB * 8 || r > CQ_MAXN || (ldS & 1))
     return false;
   cq_attrs(ctx);
@@ -1114,13 +1346,17 @@ bool launch_chol_ekf_dmma(ovb_ctx *ctx, double *S, int ldS, int r, const double 
     const int ldW = CQ_MAXN + 8;
     Lpk = ctx->d_G + (size_t)3 * ldW * ldW;
   }
-  ovb_launch(ctx, k_cq_chol_ekf, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), S, ldS, r, res, w, invdiag, ctx->d_info, Lpk, (const double *)nullptr);
+  const unsigned long long epoch = (epoch_out != nullptr && Lpk != nullptr) ? ++ctx->pub_epoch : 0;
+  ovb_launch(ctx, k_cq_chol_ekf, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), S, ldS, r, res, w, invdiag, ctx->d_info, Lpk, (const double *)nullptr,
+             epoch ? ctx->d_pub : (unsigned long long *)nullptr, epoch);
   if (Lpk_out)
     *Lpk_out = Lpk;
+  if (epoch_out)
+    *epoch_out = epoch;
   return true;
 }
 
-bool launch_trsm_rows(ovb_ctx *ctx, double *A, int ldA, int m, int nt, const double *Lpk) {
+bool launch_trsm_rows(ovb_ctx *ctx, double *A, int ldA, int m, int nt, const double *Lpk, unsigned long long epoch) {
   if (nt > CQ_MAXN || (ldA & 1) || m < 1 || Lpk == nullptr)
     return false;
   cq_attrs(ctx);
@@ -1130,7 +1366,7 @@ bool launch_trsm_rows(ovb_ctx *ctx, double *A, int ldA, int m, int nt, const dou
   int ctas = ngroups;
   if (ctas > ctx->sm_count)
     ctas = ctx->sm_count;
-  cq_launch_trsm(ctx, ctas, A, ldA, m, nt, Lpk);
+  cq_launch_trsm(ctx, ctas, A, ldA, m, nt, Lpk, epoch ? ctx->d_pub : nullptr, epoch);
   return true;
 }
 
@@ -1171,7 +1407,7 @@ static void cq_chol_blocked(ovb_ctx *ctx, double *S, int ld, int n, int extra, d
     const int nb = (n - J < CQ_WB) ? n - J : CQ_WB;
     double *Lb = Lpk + (size_t)b * CQ_PK_DOUBLES;
     ovb_launch(ctx, k_cq_chol_ekf, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), S + (size_t)J * ld + J, ld, nb, (const double *)nullptr, (double *)nullptr,
-               (double *)nullptr, info, Lb, floor_dev);
+               (double *)nullptr, info, Lb, floor_dev, (unsigned long long *)nullptr, 0ull);
     const int mrem = n + extra - (J + nb);
     if (mrem > 0) {
       double *panel = S + (size_t)(J + nb) * ld + J;
@@ -1314,11 +1550,12 @@ int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, doub
   // pass 1: G1 = A'A -> R1
   cq_launch_gram(ctx, nblk, nslab_pad, gram_smem, (const double *)A, ldA, m, nt, slab_rows, BW, nblk_side, ctx->d_Gpart, cs);
   ovb_launch(ctx, k_cq_reduce, dim3(CQ_RED_GX, nblk), dim3(CQ_RED_T), (size_t)0, (const double *)ctx->d_Gpart, npart, nblk, BW, nblk_side, nt, G, ldW, 1);
-  ovb_launch(ctx, k_cq_chol_gram, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), (const double *)G, ldW, nt, 1e-11, L1, 1);
+  const unsigned long long epoch = ++ctx->pub_epoch; // R1 streams into k_cq_solve_gram
+  ovb_launch(ctx, k_cq_chol_gram, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), (const double *)G, ldW, nt, 1e-11, L1, 1, ctx->d_pub, epoch);
   // pass 2: G2 = Q1'Q1 (one partial per slab, no cluster) -> R2
-  cq_launch_solve_gram(ctx, nslab, (const double *)A, ldA, m, nt, (const double *)L1, slab_rows, BW, ctx->d_Gpart, ctx->d_Gpart + part_doubles);
+  cq_launch_solve_gram(ctx, nslab, (const double *)A, ldA, m, nt, (const double *)L1, slab_rows, BW, ctx->d_Gpart, ctx->d_Gpart + part_doubles, ctx->d_pub, epoch);
   ovb_launch(ctx, k_cq_reduce, dim3(CQ_RED_GX, nblk), dim3(CQ_RED_T), (size_t)0, (const double *)ctx->d_Gpart, nslab, nblk, BW, nblk_side, nt, G, ldW, 1);
-  ovb_launch(ctx, k_cq_chol_gram, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), (const double *)G, ldW, nt, 1e-13, L2, 1);
+  ovb_launch(ctx, k_cq_chol_gram, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), (const double *)G, ldW, nt, 1e-13, L2, 1, (unsigned long long *)nullptr, 0ull);
   const int nT16 = (nt + 15) / 16;
   ovb_launch(ctx, k_cq_trmm, dim3(nT16, nT16), dim3(256), (size_t)0, (const double *)L2, (const double *)L1, nt, Rout, ldR);
   ctx->n_launch += 7;

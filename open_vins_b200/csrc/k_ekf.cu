@@ -442,7 +442,8 @@ void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bo
   // the residual vector is column n of H's row (TSQR output) or a separate buffer: callers stage it in d_w
   double *invdiag = ctx->d_w + ctx->cfg.max_state; // d_w holds 4 x max_state doubles: [w | 1/diag(L) | ...]
   double *Lpk = nullptr; // packed factor for the register solve (only written by the DMMA Cholesky)
-  const bool dmma_chol = ctx->ekf_chol_dmma && launch_chol_ekf_dmma(ctx, ctx->d_S, ld, r, ctx->d_w, ctx->d_w, invdiag, &Lpk);
+  unsigned long long epoch = 0; // nonzero: the factor streams into that solve
+  const bool dmma_chol = ctx->ekf_chol_dmma && launch_chol_ekf_dmma(ctx, ctx->d_S, ld, r, ctx->d_w, ctx->d_w, invdiag, &Lpk, gate_only ? nullptr : &epoch);
   // wider than one CTA's Cholesky: blocked DMMA factorisation + blocked solve (Y = M L^-T in place over M)
   const bool wide = !dmma_chol && ctx->ekf_chol_dmma && r < ld && launch_chol_solve_wide(ctx, ctx->d_S, ld, r, ctx->d_w, invdiag, ctx->d_M, ld, N, gate_only);
   if (wide) {
@@ -457,7 +458,7 @@ void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bo
   if (gate_only)
     return;
   const double *Yd = ctx->d_Y;
-  if (dmma_chol && Lpk != nullptr && launch_trsm_rows(ctx, ctx->d_M, ld, N, r, Lpk)) {
+  if (dmma_chol && Lpk != nullptr && launch_trsm_rows(ctx, ctx->d_M, ld, N, r, Lpk, epoch)) {
     Yd = ctx->d_M; // Y = M L^-T in place
   } else {
     size_t trsm_small = sizeof(double) * ((size_t)TR_ROWS * r + r);

@@ -166,6 +166,8 @@ ovb_status ovb_create(const ovb_config *cfg, ovb_ctx **out) {
   CK(cudaMalloc(&ctx->d_S, sizeof(double) * (size_t)(ms + 1) * ms));
   CK(cudaMalloc(&ctx->d_Y, sizeof(double) * (size_t)ms * ms));
   CK(cudaMalloc(&ctx->d_w, sizeof(double) * (size_t)ms * 4));
+  CK(cudaMalloc(&ctx->d_pub, sizeof(unsigned long long)));
+  CK(cudaMemset(ctx->d_pub, 0, sizeof(unsigned long long)));
   ctx->scratch_per_cta = (size_t)(2 * OVB_BIG_MAX_MEAS + 1) * (2 * OVB_BIG_MAX_MEAS + 1);
   ctx->scratch_ctas = 2 * ctx->sm_count;
   CK(cudaMalloc(&ctx->d_scratch, sizeof(double) * ctx->scratch_per_cta * ctx->scratch_ctas));
@@ -192,7 +194,7 @@ void ovb_destroy(ovb_ctx *ctx) {
     cudaStreamSynchronize(ctx->stream);
   void *dev[] = {ctx->P[0],   ctx->P[1], ctx->d_arena, ctx->d_cc, ctx->d_feat_order, ctx->d_info, ctx->d_chi2_table, ctx->d_Hs, ctx->d_W[0],
                  ctx->d_W[1], ctx->d_R,  ctx->d_R2,    ctx->d_M,  ctx->d_S,          ctx->d_Y,    ctx->d_w,          ctx->d_scratch,
-                 ctx->d_long, ctx->d_dump, ctx->P_snap, ctx->d_flush, ctx->d_Gpart, ctx->d_G, ctx->d_cqw, ctx->d_grp, ctx->d_grp_acc, ctx->d_init, ctx->d_imu};
+                 ctx->d_long, ctx->d_dump, ctx->P_snap, ctx->d_flush, ctx->d_Gpart, ctx->d_G, ctx->d_cqw, ctx->d_grp, ctx->d_grp_acc, ctx->d_init, ctx->d_imu, ctx->d_pub};
   for (void *p : dev)
     if (p)
       cudaFree(p);

@@ -211,6 +211,9 @@ struct ovb_ctx {
   size_t Gpart_cap, G_cap;
   double *d_cqw; // wide systems (k_cholqr.cu): [G1 | G2 | packed diagonal-block factors | scalars]
   size_t cqw_cap;
+  // k_cholqr.cu's factor streaming: the publication counter (device, zero at ovb_create) and the last epoch drawn
+  unsigned long long *d_pub;
+  unsigned long long pub_epoch;
   size_t last_h2d_bytes, last_d2h_bytes;
   // ovb_slam_delayed_init: the device system of the current feature and its pinned read-back (allocated on first use), and
   // the counters of the last call (ovb_last_init_counters)
@@ -264,9 +267,12 @@ int launch_compress_gram(ovb_ctx *ctx, const double *A, int m, int n, int ldA, d
 // path); returns kernels launched, or -1 when the system is too wide for it (callers then use launch_tsqr)
 int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR);
 // EKF Cholesky on the DMMA kernel of k_cholqr.cu; false when r does not fit (caller uses k_ekf_chol)
-bool launch_chol_ekf_dmma(ovb_ctx *ctx, double *S, int ldS, int r, const double *res, double *w, double *invdiag, double **Lpk_out);
-// A <- A (L')^-1 for the rows of A [m x nt] with the packed factor of the DMMA Cholesky; false when it does not fit
-bool launch_trsm_rows(ovb_ctx *ctx, double *A, int ldA, int m, int nt, const double *Lpk);
+// epoch_out != nullptr: the factor streams to the launch_trsm_rows that follows (epoch 0: it does not)
+bool launch_chol_ekf_dmma(ovb_ctx *ctx, double *S, int ldS, int r, const double *res, double *w, double *invdiag, double **Lpk_out,
+                          unsigned long long *epoch_out);
+// A <- A (L')^-1 for the rows of A [m x nt] with the packed factor of the DMMA Cholesky; false when it does not fit.
+// epoch != 0: the factor streams in from the launch_chol_ekf_dmma just before, which returned that epoch
+bool launch_trsm_rows(ovb_ctx *ctx, double *A, int ldA, int m, int nt, const double *Lpk, unsigned long long epoch);
 // wide EKF (r > 160): blocked DMMA Cholesky of S (r x r lower, residual staged in w) and Y = M L^-T in place; false when r
 // exceeds OVB_MAX_COLS or the leading dimensions are odd
 bool launch_chol_solve_wide(ovb_ctx *ctx, double *S, int ldS, int r, double *w, double *invdiag, double *M, int ldM, int N, bool gate_only);
