@@ -1187,15 +1187,151 @@ private:
 };
 
 // ---------------------------------------------------------------------------------------------------------------------
+// Filter consistency (the reference's Monte-Carlo studies: sim_save_total_state_to_file, then ov_eval's NEES and ±3σ
+// plots): per frame, the error of every base-state variable against the truth in the convention of P's error state, the
+// base block's σ, and the NEES of the IMU orientation and position (3 DOF each). The base state is one contiguous block
+// of P, ids [0, base_size): IMU 15 | dw 6 | da 6 | tg 9 | R_GYROtoIMU 3 | dt 1 | per camera: extrinsics 6, intrinsics 8.
+struct ConsistencySample {
+  double t = 0, nees_ori = 0, nees_pos = 0;
+  double cov6[21] = {0};          // upper triangle of the 6x6 [theta, p] IMU block, row by row
+  std::vector<double> err, sigma; // base_size each: truth (-) estimate, sqrt(P_ii)
+};
+
+// orientation error of a JPL quaternion in P's convention: updates are q <- dq(dtheta) ⊗ q (JPLQuat::update), so
+// q_true = dq(dtheta) ⊗ q_est gives R_true = exp(-[dtheta]x) R_est and dtheta = -log(R_true R_est')
+inline Vec3 ori_error(const Vec4 &q_true, const Vec4 &q_est) { return -log_so3(quat_2_Rot(q_true) * transpose(quat_2_Rot(q_est))); }
+
+// x' A^-1 x for the symmetric 3x3 block A of a row-major matrix with leading dimension lda, through A = L L' (no inverse);
+// NaN when the block is not positive definite
+inline double nees3(const double *A, int lda, const Vec3 &x) {
+  double L[3][3] = {{0}};
+  for (int j = 0; j < 3; j++) {
+    double d = A[(size_t)j * lda + j];
+    for (int k = 0; k < j; k++)
+      d -= L[j][k] * L[j][k];
+    if (!(d > 0))
+      return std::numeric_limits<double>::quiet_NaN();
+    L[j][j] = std::sqrt(d);
+    for (int i = j + 1; i < 3; i++) {
+      double s = A[(size_t)i * lda + j];
+      for (int k = 0; k < j; k++)
+        s -= L[i][k] * L[j][k];
+      L[i][j] = s / L[j][j];
+    }
+  }
+  double y[3], r = 0; // L y = x, then x' A^-1 x = |y|^2
+  for (int i = 0; i < 3; i++) {
+    double s = x[(size_t)i];
+    for (int k = 0; k < i; k++)
+      s -= L[i][k] * y[k];
+    y[i] = s / L[i][i];
+    r += y[i] * y[i];
+  }
+  return r;
+}
+
+// one frame: `st` after the update and the clone marginalization, `gt` = Simulator::get_state's [t q p v bg ba] at the
+// frame's IMU time, `truth` = the simulator's configuration (rpng_sim does not perturb the calibration, so the configured
+// value is the true one), P = the base block [0, base_size)^2 of the covariance, row-major
+inline ConsistencySample consistency_sample(const VioState &st, const SimParams &truth, const std::array<double, 17> &gt, const std::vector<double> &P) {
+  const int n = st.base_size;
+  ConsistencySample s;
+  s.t = st.timestamp;
+  s.err.assign((size_t)n, 0.0);
+  s.sigma.assign((size_t)n, 0.0);
+  auto put3 = [&](int id, const Vec3 &e) {
+    for (int k = 0; k < 3; k++)
+      s.err[(size_t)(id + k)] = e[(size_t)k];
+  };
+  auto diff = [&](int id, int m, const double *tru, const double *est) {
+    for (int k = 0; k < m; k++)
+      s.err[(size_t)(id + k)] = tru[k] - est[k];
+  };
+  const int i = st.imu_id;
+  put3(i, ori_error({gt[1], gt[2], gt[3], gt[4]}, st.q));
+  put3(i + 3, Vec3{gt[5], gt[6], gt[7]} - st.p);
+  put3(i + 6, Vec3{gt[8], gt[9], gt[10]} - st.v);
+  put3(i + 9, Vec3{gt[11], gt[12], gt[13]} - st.bg);
+  put3(i + 12, Vec3{gt[14], gt[15], gt[16]} - st.ba);
+  if (st.dw_id >= 0) {
+    diff(st.dw_id, 6, truth.vec_dw, st.dw);
+    diff(st.da_id, 6, truth.vec_da, st.da);
+  }
+  if (st.tg_id >= 0)
+    diff(st.tg_id, 9, truth.vec_tg, st.tg);
+  if (st.gyro_id >= 0)
+    put3(st.gyro_id, ori_error(truth.q_GYROtoIMU, st.q_GYROtoIMU));
+  if (st.dt_id >= 0)
+    diff(st.dt_id, 1, &truth.calib_camimu_dt, &st.dt_CAMtoIMU);
+  for (size_t c = 0; c < st.cams.size(); c++) {
+    const auto &cam = st.cams[c];
+    if (cam.ext_id >= 0) {
+      put3(cam.ext_id, ori_error(truth.camera_extrinsics[c].first, cam.q_ItoC));
+      put3(cam.ext_id + 3, truth.camera_extrinsics[c].second - cam.p_IinC);
+    }
+    if (cam.intr_id >= 0)
+      diff(cam.intr_id, 8, truth.camera_intrinsics[c].d, cam.intr);
+  }
+  for (int k = 0; k < n; k++)
+    s.sigma[(size_t)k] = std::sqrt(P[(size_t)k * n + k]);
+  for (int a = 0, u = 0; a < 6; a++)
+    for (int b = a; b < 6; b++)
+      s.cov6[u++] = P[(size_t)(i + a) * n + i + b];
+  s.nees_ori = nees3(P.data() + (size_t)i * n + i, n, {s.err[(size_t)i], s.err[(size_t)i + 1], s.err[(size_t)i + 2]});
+  s.nees_pos = nees3(P.data() + (size_t)(i + 3) * n + i + 3, n, {s.err[(size_t)i + 3], s.err[(size_t)i + 4], s.err[(size_t)i + 5]});
+  return s;
+}
+
+// the consistency file: a '#' header with the layout and the variable ids, then one row per frame:
+// t nees_ori nees_pos cov6[21] err[n] sigma[n]
+inline void write_consistency_file(const std::string &path, const VioState &st, const std::vector<ConsistencySample> &rows) {
+  FILE *f = std::fopen(path.c_str(), "w");
+  if (!f)
+    return;
+  std::fprintf(f, "# t nees_ori nees_pos cov6[21] err[n] sigma[n] | cov6: upper triangle of the [theta p] IMU block, row by row | err: truth - "
+                  "estimate, orientations -log(R_true R_est') | ids: imu=%d",
+               st.imu_id);
+  if (st.dw_id >= 0)
+    std::fprintf(f, " dw=%d da=%d", st.dw_id, st.da_id);
+  if (st.tg_id >= 0)
+    std::fprintf(f, " tg=%d", st.tg_id);
+  if (st.gyro_id >= 0)
+    std::fprintf(f, " gyro=%d", st.gyro_id);
+  if (st.dt_id >= 0)
+    std::fprintf(f, " dt=%d", st.dt_id);
+  for (size_t c = 0; c < st.cams.size(); c++) {
+    if (st.cams[c].ext_id >= 0)
+      std::fprintf(f, " cam%zu_ext=%d", c, st.cams[c].ext_id);
+    if (st.cams[c].intr_id >= 0)
+      std::fprintf(f, " cam%zu_intr=%d", c, st.cams[c].intr_id);
+  }
+  std::fprintf(f, " n=%d\n", st.base_size);
+  for (const auto &r : rows) {
+    std::fprintf(f, "%.9f %.17g %.17g", r.t, r.nees_ori, r.nees_pos);
+    for (double x : r.cov6)
+      std::fprintf(f, " %.17g", x);
+    for (double x : r.err)
+      std::fprintf(f, " %.17g", x);
+    for (double x : r.sigma)
+      std::fprintf(f, " %.17g", x);
+    std::fprintf(f, "\n");
+  }
+  std::fclose(f);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // run_simulation main loop (ov_msckf/src/run_simulation.cpp:117-176): initialise from the simulator's ground truth, feed
 // IMU at sim_freq_imu and camera frames with the reference's one-frame delay buffer. Stops after max_frames camera updates
 // (0 = whole trajectory). Ground truth samples are taken at the estimate's timestamps (+dt) from the simulator's spline.
+// record_consistency: after every frame, outside the frame's timed region, read the base block of P (one
+// get_marginal) and append a ConsistencySample; off, the loop makes exactly the backend calls it makes without it.
 struct SimRunResult {
   std::vector<TrajSample> est, gt;
   double ate_ori_deg = 0, ate_pos = 0;
   int frames = 0;
+  std::vector<ConsistencySample> consistency;
 };
-inline SimRunResult run_simulation(Simulator &sim, VioManager &sys, int max_frames = 0) {
+inline SimRunResult run_simulation(Simulator &sim, VioManager &sys, int max_frames = 0, bool record_consistency = false) {
   const double next_imu_time = sim.current_timestamp() + 1.0 / sim.params.sim_freq_imu;
   std::array<double, 17> imustate;
   if (!sim.get_state(next_imu_time, imustate))
@@ -1220,10 +1356,18 @@ inline SimRunResult run_simulation(Simulator &sim, VioManager &sys, int max_fram
         if (sys.trajectory_est.size() > before) {
           std::array<double, 17> gt;
           const TrajSample &e = sys.trajectory_est.back();
-          if (sim.get_state(e.t + sim.params.calib_camimu_dt, gt))
+          const bool have_gt = sim.get_state(e.t + sim.params.calib_camimu_dt, gt);
+          if (have_gt)
             res.gt.push_back({e.t, {gt[1], gt[2], gt[3], gt[4]}, {gt[5], gt[6], gt[7]}});
           else
             res.gt.push_back(e);
+          if (record_consistency) {
+            const VioState &st = sys.state;
+            if (!have_gt) // past the trajectory's end: like the ATE, the estimate stands in for the truth
+              gt = {st.timestamp, st.q[0], st.q[1], st.q[2], st.q[3], st.p[0], st.p[1], st.p[2], st.v[0], st.v[1], st.v[2],
+                    st.bg[0], st.bg[1], st.bg[2], st.ba[0], st.ba[1], st.ba[2]};
+            res.consistency.push_back(consistency_sample(st, sim.params, gt, sys.cov->get_marginal({0}, {st.base_size})));
+          }
         }
         if (max_frames > 0 && sys.frames_done >= max_frames)
           break;

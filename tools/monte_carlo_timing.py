@@ -13,6 +13,12 @@ that made it. A reallocation frees first, and cudaFree waits for the whole devic
 would stall the other runs of a batch.
 
   python tools/monte_carlo_timing.py [--ks 1,2,4,8,16] [--out FILE]
+  python tools/monte_carlo_timing.py --consistency ab --ks 1,16 [--reps 3]
+
+--consistency on runs every batch with --consistency (per frame, one read of the covariance's base block and its
+synchronisation, the errors and NEES, and DIR/consistency_<seed>.txt). --consistency ab measures its cost: for each shape
+and K, --reps rounds of both arms back to back, the order alternating from round to round; both arms write their estimate
+files to a temporary --out-dir, so the difference is the consistency recording alone. The growth probe is skipped.
 
 Prints one JSON line per measurement, the card's name, power limit and max SM clock among them. Needs a GPU; there is no
 CPU path."""
@@ -51,14 +57,20 @@ def runner_cmd(exe, shape):
             str(s["pts"]), "--frames", str(s["frames"])]
 
 
-def time_batch(exe, shape, k):
+def time_batch(exe, shape, k, consistency=False, out_dir=None):
+    extra = (["--consistency"] if consistency else []) + (["--out-dir", out_dir] if out_dir else [])
     t0 = time.perf_counter()
-    out = subprocess.run(runner_cmd(exe, shape) + ["--runs", str(k), "--jobs", str(k)], check=True, capture_output=True, text=True).stdout
+    out = subprocess.run(runner_cmd(exe, shape) + ["--runs", str(k), "--jobs", str(k)] + extra, check=True, capture_output=True, text=True).stdout
     wall = time.perf_counter() - t0
     r = json.loads(out.strip().splitlines()[-1])
-    return dict(tool="monte_carlo_timing", shape=shape, runs=k, jobs=r["jobs"], frames_total=r["frames_total"], process_s=wall,
-                runs_per_s=k / wall, frames_per_s=r["frames_total"] / wall, runner_wall_s=r["wall_s"], runner_runs_per_s=r["runs_per_s"],
-                ate_pos_m_mean=r["ate_pos_m_mean"], ate_pos_m_std=r["ate_pos_m_std"])
+    rec = dict(tool="monte_carlo_timing", shape=shape, runs=k, jobs=r["jobs"], frames_total=r["frames_total"], process_s=wall,
+               runs_per_s=k / wall, frames_per_s=r["frames_total"] / wall, runner_wall_s=r["wall_s"], runner_runs_per_s=r["runs_per_s"],
+               ate_pos_m_mean=r["ate_pos_m_mean"], ate_pos_m_std=r["ate_pos_m_std"])
+    if consistency:
+        rec.update(consistency=True, runner_frames_per_s=r["frames_per_s"], nees_ori_mean=r["nees_ori_mean"], nees_pos_mean=r["nees_pos_mean"])
+    elif out_dir:
+        rec.update(consistency=False, runner_frames_per_s=r["frames_per_s"])
+    return rec
 
 
 def text_symbols(lib):
@@ -104,6 +116,8 @@ def main():
     ap.add_argument("--ks", default="1,2,4,8,16")
     ap.add_argument("--shapes", default=",".join(SHAPES))
     ap.add_argument("--out", default=None, help="also write the JSON lines to this file")
+    ap.add_argument("--consistency", choices=["off", "on", "ab"], default="off", help="record consistency in every batch, or A/B it")
+    ap.add_argument("--reps", type=int, default=3, help="rounds of both arms per shape and K with --consistency ab")
     a = ap.parse_args()
     exe = b.build_sim_tools()
     recs = [dict(tool="monte_carlo_timing", gpu=gpu_info())]
@@ -112,10 +126,18 @@ def main():
         for shape in a.shapes.split(","):
             subprocess.run(runner_cmd(exe, shape)[:-2] + ["--frames", "20"], check=True, capture_output=True)  # warm-up: driver, page cache
             for k in [int(x) for x in a.ks.split(",")]:
-                recs.append(time_batch(exe, shape, k))
+                if a.consistency != "ab":
+                    recs.append(time_batch(exe, shape, k, consistency=a.consistency == "on"))
+                    print(json.dumps(recs[-1]), flush=True)
+                    continue
+                for rep in range(a.reps):
+                    for arm in ((False, True) if rep % 2 == 0 else (True, False)):
+                        d = tempfile.mkdtemp(dir=tmp)
+                        recs.append(dict(time_batch(exe, shape, k, consistency=arm, out_dir=d), rep=rep))
+                        print(json.dumps(recs[-1]), flush=True)
+            if a.consistency != "ab":
+                recs.append(probe_growth(exe, shape, tmp))
                 print(json.dumps(recs[-1]), flush=True)
-            recs.append(probe_growth(exe, shape, tmp))
-            print(json.dumps(recs[-1]), flush=True)
     recs.append(dict(tool="monte_carlo_timing", gpu_after=gpu_info()))
     print(json.dumps(recs[-1]), flush=True)
     if a.out:

@@ -4,8 +4,12 @@
 //   -DOVB_SIM_HOST_PROPAGATION (test infrastructure): the engine with the IMU covariance accumulation on the host
 // Usage: <exe> --traj FILE(.txt|.bin) [--cams K] [--clones C] [--msckf M] [--pts P] [--frames F] [--calib 0|1]
 //              [--est OUT.txt] [--timing [OUT.csv]] [--capture FRAME PREFIX] [--integration discrete|rk4|analytical]
-//              [--seed-init S] [--seed-perturb S] [--seed-meas S] [--runs K [--jobs J] [--out-dir DIR]]
+//              [--seed-init S] [--seed-perturb S] [--seed-meas S] [--runs K [--jobs J] [--out-dir DIR]] [--consistency [OUT.txt]]
 // Prints one JSON line: frames, ATE (alignment none), mean per-stage host times.
+// --consistency OUT.txt: after every frame, read the base block of the covariance and write one row of errors against the
+// truth, σ and the orientation / position NEES (write_consistency_file in include/ovb200_vio.hpp; INTEGRATION.md §8); the
+// JSON line gains the run's mean nees_ori and nees_pos. With --runs, --consistency takes no path: DIR/consistency_<seed>.txt
+// per run, nees_ori / nees_pos per run and their mean and population standard deviation over the runs.
 // --runs K: a Monte-Carlo batch of K runs in this process, run r with measurement seed seed_meas + r (same map and initial
 // state, different noise). J host threads (default min(K, hardware threads)) take runs from a shared counter; each run owns
 // its Simulator, VioManager and backend (with the engine: its own ovb_ctx on device 0), so a run computes the same bits
@@ -40,6 +44,7 @@ struct RunnerOptions {
 struct RunSummary {
   int frames = 0, state_dim = 0;
   double ate_pos = 0, ate_ori_deg = 0, feats_in = 0, feats_used = 0, rows = 0, ms_prop = 0, ms_msckf = 0, ms_total = 0;
+  double nees_ori = 0, nees_pos = 0; // means over the run's frames (with --consistency)
   size_t map_points = 0;
   long status_hist[9] = {0};
 };
@@ -50,9 +55,11 @@ static const char *const backend_name = "oracle";
 static const char *const backend_name = "engine";
 #endif
 
-// one closed-loop run with measurement seed `seed_meas`; empty paths write nothing, capture_frame < 0 captures nothing
+// one closed-loop run with measurement seed `seed_meas`; empty paths write nothing, capture_frame < 0 captures nothing,
+// consistency = record the consistency samples (written to consistency_path unless it is empty)
 static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<double, 8>> &traj_data, int seed_meas, const std::string &est_path,
-                          const std::string &timing_path, int capture_frame, const std::string &capture_prefix) {
+                          const std::string &timing_path, bool consistency, const std::string &consistency_path, int capture_frame,
+                          const std::string &capture_prefix) {
   SimParams sp;
   rpng_sim_cameras(o.cams, sp);
   sp.use_stereo = o.cams > 1;
@@ -117,7 +124,7 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
       std::fclose(f);
     };
   }
-  SimRunResult res = run_simulation(sim, sys, o.frames);
+  SimRunResult res = run_simulation(sim, sys, o.frames, consistency);
   if (!est_path.empty()) {
     FILE *f = std::fopen(est_path.c_str(), "w");
     if (f) {
@@ -133,6 +140,8 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
   }
   if (!timing_path.empty())
     sys.write_timing_csv(timing_path);
+  if (!consistency_path.empty())
+    write_consistency_file(consistency_path, sys.state, res.consistency);
   double t_prop = 0, t_msckf = 0, t_total = 0, feats = 0, used = 0, rows = 0;
   for (const auto &t : sys.timing) {
     t_prop += t.time_prop, t_msckf += t.time_msckf, t_total += t.time_total;
@@ -148,11 +157,16 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
   s.map_points = sim.featmap.size();
   for (int k = 0; k < 9; k++)
     s.status_hist[k] = sys.status_hist[k];
+  for (const auto &c : res.consistency)
+    s.nees_ori += c.nees_ori, s.nees_pos += c.nees_pos;
+  if (!res.consistency.empty())
+    s.nees_ori /= (double)res.consistency.size(), s.nees_pos /= (double)res.consistency.size();
   return s;
 }
 
 // the --runs batch: returns the process exit code
-static int run_batch(const RunnerOptions &o, const std::vector<std::array<double, 8>> &traj_data, int runs, int jobs, const std::string &out_dir, bool timing) {
+static int run_batch(const RunnerOptions &o, const std::vector<std::array<double, 8>> &traj_data, int runs, int jobs, const std::string &out_dir, bool timing,
+                     bool consistency) {
   std::vector<RunSummary> out((size_t)runs);
   std::vector<std::string> err((size_t)runs);
   std::atomic<int> next{0};
@@ -163,7 +177,8 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
       const std::string stem = out_dir.empty() ? std::string() : out_dir + "/";
       try {
         out[(size_t)r] = run_one(o, traj_data, seed, stem.empty() ? "" : stem + "est_" + std::to_string(seed) + ".txt",
-                                 stem.empty() || !timing ? "" : stem + "timing_" + std::to_string(seed) + ".csv", -1, "");
+                                 stem.empty() || !timing ? "" : stem + "timing_" + std::to_string(seed) + ".csv", consistency,
+                                 stem.empty() || !consistency ? "" : stem + "consistency_" + std::to_string(seed) + ".txt", -1, "");
       } catch (const std::exception &e) {
         err[(size_t)r] = e.what();
         failed = true; // the runs already started finish; no new one starts
@@ -198,25 +213,44 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
   for (int r = 0; r < runs; r++) {
     const RunSummary &s = out[(size_t)r];
     char buf[512];
-    std::snprintf(buf, sizeof(buf), "%s{\"seed\": %d, \"frames\": %d, \"ate_pos_m\": %.17g, \"ate_ori_deg\": %.17g, \"status_hist\": [%ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld]}",
+    std::snprintf(buf, sizeof(buf), "%s{\"seed\": %d, \"frames\": %d, \"ate_pos_m\": %.17g, \"ate_ori_deg\": %.17g, \"status_hist\": [%ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld]",
                   r ? ", " : "", o.seed_meas + r, s.frames, s.ate_pos, s.ate_ori_deg, s.status_hist[0], s.status_hist[1], s.status_hist[2], s.status_hist[3],
                   s.status_hist[4], s.status_hist[5], s.status_hist[6], s.status_hist[7], s.status_hist[8]);
     per_run += buf;
+    if (consistency) {
+      std::snprintf(buf, sizeof(buf), ", \"nees_ori\": %.17g, \"nees_pos\": %.17g", s.nees_ori, s.nees_pos);
+      per_run += buf;
+    }
+    per_run += "}";
+  }
+  // the same statistics of the per-run mean NEES
+  std::string nees;
+  if (consistency) {
+    double no = 0, np = 0, vno = 0, vnp = 0;
+    for (const auto &s : out)
+      no += s.nees_ori, np += s.nees_pos;
+    no /= runs, np /= runs;
+    for (const auto &s : out)
+      vno += (s.nees_ori - no) * (s.nees_ori - no), vnp += (s.nees_pos - np) * (s.nees_pos - np);
+    char buf[256];
+    std::snprintf(buf, sizeof(buf), ", \"nees_ori_mean\": %.17g, \"nees_ori_std\": %.17g, \"nees_pos_mean\": %.17g, \"nees_pos_std\": %.17g", no,
+                  std::sqrt(vno / runs), np, std::sqrt(vnp / runs));
+    nees = buf;
   }
   std::printf("{\"backend\": \"%s\", \"runs\": %d, \"jobs\": %d, \"cams\": %d, \"max_clones\": %d, \"max_msckf_in_update\": %d, \"num_pts\": %d, \"calib\": %d, "
               "\"seed_init\": %d, \"seed_perturb\": %d, \"seed_meas\": %d, \"state_dim\": %d, \"map_points\": %zu, \"per_run\": [%s], "
               "\"ate_pos_m_mean\": %.17g, \"ate_pos_m_std\": %.17g, \"ate_ori_deg_mean\": %.17g, \"ate_ori_deg_std\": %.17g, \"frames_total\": %ld, "
-              "\"wall_s\": %.6f, \"runs_per_s\": %.6f, \"frames_per_s\": %.3f}\n",
+              "\"wall_s\": %.6f, \"runs_per_s\": %.6f, \"frames_per_s\": %.3f%s}\n",
               backend_name, runs, jobs, o.cams, o.clones, o.msckf, o.pts, o.calib, o.seed_init, o.seed_perturb, o.seed_meas, out[0].state_dim, out[0].map_points,
-              per_run.c_str(), mp, std::sqrt(vp / runs), mo, std::sqrt(vo / runs), frames, wall, runs / wall, frames / wall);
+              per_run.c_str(), mp, std::sqrt(vp / runs), mo, std::sqrt(vo / runs), frames, wall, runs / wall, frames / wall, nees.c_str());
   return 0;
 }
 
 int main(int argc, char **argv) {
   RunnerOptions o;
-  std::string est_path, timing_path, capture_prefix, out_dir;
+  std::string est_path, timing_path, consistency_path, capture_prefix, out_dir;
   int capture_frame = -1, runs = 0, jobs = 0;
-  bool timing = false;
+  bool timing = false, consistency = false;
   for (int i = 1; i < argc; i++) {
     auto next = [&]() { return std::string(i + 1 < argc ? argv[++i] : ""); };
     const std::string a = argv[i];
@@ -233,6 +267,11 @@ int main(int argc, char **argv) {
       if (i + 1 < argc && std::strncmp(argv[i + 1], "--", 2) != 0)
         timing_path = next();
     }
+    else if (a == "--consistency") { // like --timing: a --runs batch names its files itself
+      consistency = true;
+      if (i + 1 < argc && std::strncmp(argv[i + 1], "--", 2) != 0)
+        consistency_path = next();
+    }
     else if (a == "--integration") o.integration = next();
     else if (a == "--compress") o.compress = next();
     else if (a == "--capture") { capture_frame = std::stoi(next()); capture_prefix = next(); }
@@ -245,6 +284,10 @@ int main(int argc, char **argv) {
   }
   if (runs < 0 || jobs < 0 || (runs == 0 && (jobs > 0 || !out_dir.empty())) || (runs > 0 && (!est_path.empty() || capture_frame >= 0))) {
     std::fprintf(stderr, "--runs K takes --jobs J >= 1 and --out-dir DIR; --jobs and --out-dir need --runs; --est and --capture are single-run options\n");
+    return 2;
+  }
+  if (consistency && runs == 0 && consistency_path.empty()) {
+    std::fprintf(stderr, "--consistency takes the output file's path on a single run (a --runs batch writes DIR/consistency_<seed>.txt)\n");
     return 2;
   }
   std::vector<std::array<double, 8>> traj_data =
@@ -265,16 +308,19 @@ int main(int argc, char **argv) {
         return 2;
       }
     }
-    return run_batch(o, traj_data, runs, jobs, out_dir, timing);
+    return run_batch(o, traj_data, runs, jobs, out_dir, timing, consistency);
   }
   try {
-    const RunSummary s = run_one(o, traj_data, o.seed_meas, est_path, timing_path, capture_frame, capture_prefix);
+    const RunSummary s = run_one(o, traj_data, o.seed_meas, est_path, timing_path, consistency, consistency_path, capture_frame, capture_prefix);
+    char nees[128] = "";
+    if (consistency)
+      std::snprintf(nees, sizeof(nees), ", \"nees_ori\": %.12g, \"nees_pos\": %.12g", s.nees_ori, s.nees_pos);
     std::printf("{\"backend\": \"%s\", \"frames\": %d, \"cams\": %d, \"max_clones\": %d, \"max_msckf_in_update\": %d, \"num_pts\": %d, \"calib\": %d, "
                 "\"state_dim\": %d, \"ate_pos_m\": %.12g, \"ate_ori_deg\": %.12g, \"mean_feats_in\": %.2f, \"mean_feats_used\": %.2f, \"mean_rows\": %.1f, "
-                "\"mean_ms_propagation\": %.4f, \"mean_ms_msckf_update\": %.4f, \"mean_ms_total\": %.4f, \"map_points\": %zu, \"status_hist\": [%ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld]}\n",
+                "\"mean_ms_propagation\": %.4f, \"mean_ms_msckf_update\": %.4f, \"mean_ms_total\": %.4f, \"map_points\": %zu, \"status_hist\": [%ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld]%s}\n",
                 backend_name, s.frames, o.cams, o.clones, o.msckf, o.pts, o.calib, s.state_dim, s.ate_pos, s.ate_ori_deg, s.feats_in, s.feats_used, s.rows,
                 s.ms_prop, s.ms_msckf, s.ms_total, s.map_points, s.status_hist[0], s.status_hist[1], s.status_hist[2], s.status_hist[3], s.status_hist[4],
-                s.status_hist[5], s.status_hist[6], s.status_hist[7], s.status_hist[8]);
+                s.status_hist[5], s.status_hist[6], s.status_hist[7], s.status_hist[8], nees);
   } catch (const std::exception &e) {
     std::fprintf(stderr, "run_simulation failed: %s\n", e.what());
     return 1;
