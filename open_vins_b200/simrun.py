@@ -23,7 +23,8 @@ CASE_CONFIG2 = os.path.join(os.path.dirname(HERE), "tests", "golden", "rpng_sim_
 
 
 def run(exe=None, traj=None, cams=2, clones=11, msckf=10, pts=250, frames=0, calib=1, est=None, timing=None, capture=None, integration="rk4",
-        compress="cholqr2", seed_init=0, seed_perturb=0, seed_meas=0, runs=None, jobs=None, out_dir=None, consistency=None, timeout=1800):
+        compress="cholqr2", seed_init=0, seed_perturb=0, seed_meas=0, runs=None, jobs=None, out_dir=None, consistency=None, cam_model=None,
+        timeout=1800):
     """Runs the simulation; returns the parsed JSON summary. capture = (frame_index, path_prefix) dumps that update's inputs.
     seed_init / seed_perturb / seed_meas: the simulator's random seeds (rpng_sim's sim_seed_state_init, sim_seed_preturb,
     sim_seed_measurements). runs = K: a Monte-Carlo batch in one process, run r with measurement seed seed_meas + r, on
@@ -31,7 +32,9 @@ def run(exe=None, traj=None, cams=2, clones=11, msckf=10, pts=250, frames=0, cal
     truthy, timing_<seed>.csv. The batch summary lists every run under "per_run" with the mean and population standard
     deviation of both ATEs. consistency = PATH (single run) or True (batch; out_dir receives consistency_<seed>.txt): record
     the per-frame errors, σ and NEES (load_consistency); the summary gains the mean nees_ori / nees_pos, per run in a batch
-    with their mean and population standard deviation over the runs."""
+    with their mean and population standard deviation over the runs. cam_model = "radtan" or "equi" for every camera, or a
+    sequence with one model per camera (a mixed rig): equidistant cameras take the TUM-VI cam0 intrinsics on a 512 x 512
+    image (INTEGRATION.md §8), and the summary gains "cam_model". None runs the rpng_sim radtan cameras."""
     cmd = [exe or ENGINE_EXE, "--traj", traj or TRAJ_FIXTURE, "--cams", str(cams), "--clones", str(clones), "--msckf", str(msckf), "--pts", str(pts),
            "--frames", str(frames), "--calib", str(int(calib)), "--integration", integration, "--compress", compress,
            "--seed-init", str(seed_init), "--seed-perturb", str(seed_perturb), "--seed-meas", str(seed_meas)]
@@ -41,6 +44,8 @@ def run(exe=None, traj=None, cams=2, clones=11, msckf=10, pts=250, frames=0, cal
         cmd += ["--timing"] if runs else ["--timing", timing]
     if consistency:
         cmd += ["--consistency"] if runs or consistency is True else ["--consistency", str(consistency)]
+    if cam_model is not None:
+        cmd += ["--cam-model", cam_model if isinstance(cam_model, str) else ",".join(cam_model)]
     if capture:
         cmd += ["--capture", str(capture[0]), capture[1]]
     if runs:

@@ -5,7 +5,12 @@
 // Usage: <exe> --traj FILE(.txt|.bin) [--cams K] [--clones C] [--msckf M] [--pts P] [--frames F] [--calib 0|1]
 //              [--est OUT.txt] [--timing [OUT.csv]] [--capture FRAME PREFIX] [--integration discrete|rk4|analytical]
 //              [--seed-init S] [--seed-perturb S] [--seed-meas S] [--runs K [--jobs J] [--out-dir DIR]] [--consistency [OUT.txt]]
+//              [--cam-model M[,M...]]
 // Prints one JSON line: frames, ATE (alignment none), mean per-stage host times.
+// --cam-model radtan|equi: the camera model of every camera, or one per camera (a mixed rig, e.g. radtan,equi). Equidistant
+// cameras take the TUM-VI cam0 intrinsics on a 512 x 512 image and the rpng_sim extrinsics of their slot (rpng_sim_cameras
+// in include/ovb200_sim.hpp); the JSON line gains "cam_model", one entry per camera. Without the flag every camera is the
+// rpng_sim radtan camera.
 // --consistency OUT.txt: after every frame, read the base block of the covariance and write one row of errors against the
 // truth, σ and the orientation / position NEES (write_consistency_file in include/ovb200_vio.hpp; INTEGRATION.md §8); the
 // JSON line gains the run's mean nees_ori and nees_pos. With --runs, --consistency takes no path: DIR/consistency_<seed>.txt
@@ -38,7 +43,40 @@ struct RunnerOptions {
   std::string traj, integration = "rk4", compress = "cholqr2";
   int cams = 2, clones = 11, msckf = 10, pts = 250, frames = 0, calib = 1;
   int seed_init = 0, seed_perturb = 0, seed_meas = 0;
+  std::vector<int> cam_models; // per camera (--cam-model); empty = all radtan
 };
+
+// the JSON field of --cam-model (empty without the flag): , "cam_model": ["radtan", "equi", ...]
+static std::string cam_model_json(const RunnerOptions &o) {
+  if (o.cam_models.empty())
+    return "";
+  std::string s = ", \"cam_model\": [";
+  for (size_t k = 0; k < o.cam_models.size(); k++)
+    s += std::string(k ? ", " : "") + (o.cam_models[k] == OVB_CAM_EQUI ? "\"equi\"" : "\"radtan\"");
+  return s + "]";
+}
+
+// --cam-model M[,M...] for `cams` cameras: false on an unknown model or a count other than 1 or cams
+static bool parse_cam_models(const std::string &arg, int cams, std::vector<int> &out) {
+  out.clear();
+  size_t a = 0;
+  while (true) {
+    const size_t b = arg.find(',', a);
+    const std::string m = arg.substr(a, b == std::string::npos ? std::string::npos : b - a);
+    if (m == "radtan")
+      out.push_back(OVB_CAM_RADTAN);
+    else if (m == "equi")
+      out.push_back(OVB_CAM_EQUI);
+    else
+      return false;
+    if (b == std::string::npos)
+      break;
+    a = b + 1;
+  }
+  if (out.size() == 1)
+    out.assign((size_t)std::max(cams, 1), out[0]);
+  return (int)out.size() == cams;
+}
 
 // what one run reports (the single-run JSON line, and one entry of a --runs batch)
 struct RunSummary {
@@ -61,7 +99,7 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
                           const std::string &timing_path, bool consistency, const std::string &consistency_path, int capture_frame,
                           const std::string &capture_prefix) {
   SimParams sp;
-  rpng_sim_cameras(o.cams, sp);
+  rpng_sim_cameras(o.cams, sp, o.cam_models);
   sp.use_stereo = o.cams > 1;
   sp.num_pts = o.pts;
   sp.seed_state_init = o.seed_init;
@@ -237,20 +275,20 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
                   std::sqrt(vno / runs), np, std::sqrt(vnp / runs));
     nees = buf;
   }
-  std::printf("{\"backend\": \"%s\", \"runs\": %d, \"jobs\": %d, \"cams\": %d, \"max_clones\": %d, \"max_msckf_in_update\": %d, \"num_pts\": %d, \"calib\": %d, "
+  std::printf("{\"backend\": \"%s\", \"runs\": %d, \"jobs\": %d, \"cams\": %d%s, \"max_clones\": %d, \"max_msckf_in_update\": %d, \"num_pts\": %d, \"calib\": %d, "
               "\"seed_init\": %d, \"seed_perturb\": %d, \"seed_meas\": %d, \"state_dim\": %d, \"map_points\": %zu, \"per_run\": [%s], "
               "\"ate_pos_m_mean\": %.17g, \"ate_pos_m_std\": %.17g, \"ate_ori_deg_mean\": %.17g, \"ate_ori_deg_std\": %.17g, \"frames_total\": %ld, "
               "\"wall_s\": %.6f, \"runs_per_s\": %.6f, \"frames_per_s\": %.3f%s}\n",
-              backend_name, runs, jobs, o.cams, o.clones, o.msckf, o.pts, o.calib, o.seed_init, o.seed_perturb, o.seed_meas, out[0].state_dim, out[0].map_points,
+              backend_name, runs, jobs, o.cams, cam_model_json(o).c_str(), o.clones, o.msckf, o.pts, o.calib, o.seed_init, o.seed_perturb, o.seed_meas, out[0].state_dim, out[0].map_points,
               per_run.c_str(), mp, std::sqrt(vp / runs), mo, std::sqrt(vo / runs), frames, wall, runs / wall, frames / wall, nees.c_str());
   return 0;
 }
 
 int main(int argc, char **argv) {
   RunnerOptions o;
-  std::string est_path, timing_path, consistency_path, capture_prefix, out_dir;
+  std::string est_path, timing_path, consistency_path, capture_prefix, out_dir, cam_model_arg;
   int capture_frame = -1, runs = 0, jobs = 0;
-  bool timing = false, consistency = false;
+  bool timing = false, consistency = false, cam_model = false;
   for (int i = 1; i < argc; i++) {
     auto next = [&]() { return std::string(i + 1 < argc ? argv[++i] : ""); };
     const std::string a = argv[i];
@@ -281,9 +319,15 @@ int main(int argc, char **argv) {
     else if (a == "--runs") runs = std::stoi(next());
     else if (a == "--jobs") jobs = std::stoi(next());
     else if (a == "--out-dir") out_dir = next();
+    else if (a == "--cam-model") { cam_model = true; cam_model_arg = next(); }
   }
   if (runs < 0 || jobs < 0 || (runs == 0 && (jobs > 0 || !out_dir.empty())) || (runs > 0 && (!est_path.empty() || capture_frame >= 0))) {
     std::fprintf(stderr, "--runs K takes --jobs J >= 1 and --out-dir DIR; --jobs and --out-dir need --runs; --est and --capture are single-run options\n");
+    return 2;
+  }
+  if (cam_model && !parse_cam_models(cam_model_arg, o.cams, o.cam_models)) {
+    std::fprintf(stderr, "--cam-model takes radtan or equi, once for every camera or once per camera (--cams %d), not '%s'\n", o.cams,
+                 cam_model_arg.c_str());
     return 2;
   }
   if (consistency && runs == 0 && consistency_path.empty()) {
@@ -315,10 +359,10 @@ int main(int argc, char **argv) {
     char nees[128] = "";
     if (consistency)
       std::snprintf(nees, sizeof(nees), ", \"nees_ori\": %.12g, \"nees_pos\": %.12g", s.nees_ori, s.nees_pos);
-    std::printf("{\"backend\": \"%s\", \"frames\": %d, \"cams\": %d, \"max_clones\": %d, \"max_msckf_in_update\": %d, \"num_pts\": %d, \"calib\": %d, "
+    std::printf("{\"backend\": \"%s\", \"frames\": %d, \"cams\": %d%s, \"max_clones\": %d, \"max_msckf_in_update\": %d, \"num_pts\": %d, \"calib\": %d, "
                 "\"state_dim\": %d, \"ate_pos_m\": %.12g, \"ate_ori_deg\": %.12g, \"mean_feats_in\": %.2f, \"mean_feats_used\": %.2f, \"mean_rows\": %.1f, "
                 "\"mean_ms_propagation\": %.4f, \"mean_ms_msckf_update\": %.4f, \"mean_ms_total\": %.4f, \"map_points\": %zu, \"status_hist\": [%ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld]%s}\n",
-                backend_name, s.frames, o.cams, o.clones, o.msckf, o.pts, o.calib, s.state_dim, s.ate_pos, s.ate_ori_deg, s.feats_in, s.feats_used, s.rows,
+                backend_name, s.frames, o.cams, cam_model_json(o).c_str(), o.clones, o.msckf, o.pts, o.calib, s.state_dim, s.ate_pos, s.ate_ori_deg, s.feats_in, s.feats_used, s.rows,
                 s.ms_prop, s.ms_msckf, s.ms_total, s.map_points, s.status_hist[0], s.status_hist[1], s.status_hist[2], s.status_hist[3], s.status_hist[4],
                 s.status_hist[5], s.status_hist[6], s.status_hist[7], s.status_hist[8], nees);
   } catch (const std::exception &e) {
