@@ -338,6 +338,51 @@ ovb_status ovb_slam_anchor_change(const ovb_frame *frame, const ovb_opts *opts, 
                                   int old_cam, int old_clone, int new_cam, int new_clone, double *new_value, double *new_value_fej,
                                   double *Phi, int32_t *order_off, int32_t *order_sz, int32_t *n_order, int32_t *n_cols);
 
+/* The landmarks ovb_marginalize_window re-anchors (UpdaterSLAM::change_anchors), one entry per landmark, in the order the
+ * anchor changes are applied. */
+typedef struct {
+  int n;                             /* landmarks to re-anchor */
+  const int32_t *lm_off;             /* [n] covariance id (3 wide; 1 for ANCHORED_INVERSE_DEPTH_SINGLE) */
+  const int32_t *feat_rep;           /* [n] an anchored ovb_feat_rep */
+  const double *value, *value_fej;   /* [n][3] Landmark::get_xyz(false / true) */
+  const int32_t *old_cam, *old_clone, *new_cam, *new_clone; /* [n] camera ids and clone indices into the frame */
+  double *new_value, *new_value_fej; /* [n][3] out: Landmark::set_from_xyz in the new anchor */
+} ovb_anchor_changes;
+
+/* The covariance side of the end of VioManager::do_feature_propagate_update in one call: StateHelper::marginalize_slam,
+ * UpdaterSLAM::change_anchors and StateHelper::marginalize_old_clone (VioManager::do_feature_propagate_update). The n_marg ranges
+ * (marg_off[i], marg_sz[i]) are the lost landmarks and the oldest clone; anchors (or NULL) the landmarks to re-anchor, with
+ * ovb_opts' do_fej and do_calib_camera_pose. All offsets refer to the covariance before the call; afterwards N shrinks by
+ * the ranges' total and the host shifts its Type::id()s exactly as it does after each ovb_cov_marginalize.
+ * Result: P and N are those of this sequence of existing calls: every anchor change in the order given
+ * (ovb_slam_anchor_change, then ovb_cov_propagate with Q = 0), then ovb_cov_marginalize of every range, highest offset first.
+ * P, new_value and new_value_fej are bit-identical to that sequence for every anchored representation. The anchor-change
+ * math of ANCHORED_3D, ANCHORED_MSCKF_INVERSE_DEPTH and ANCHORED_INVERSE_DEPTH_SINGLE runs on the device from the same source
+ * as ovb_slam_anchor_change, built without FMA contraction for both sides. An ANCHORED_FULL_INVERSE_DEPTH landmark's Phi
+ * goes through acos, atan2, sin and cos, whose CUDA and C-library results may differ in the last ulp, so the call computes
+ * that Phi with ovb_slam_anchor_change on the host and uploads it with the other inputs.
+ * Whether the lost landmarks are marginalized before or after the anchor changes (the reference calls marginalize_slam
+ * and change_anchors in either order, both before marginalize_old_clone) does not change a bit when P is symmetric, as the
+ * filter's covariance is: marginalization only copies entries (some read from the mirrored position, which holds the same
+ * value), an anchor change writes only the rows and columns of its own landmark and reads only those and the ones of its
+ * anchor clones and extrinsics, none of which a marginalization removes (a landmark may not be both re-anchored and
+ * marginalized; the old anchor clone is read before marginalize_old_clone drops it, in both orders).
+ * Everything is checked before any work is enqueued; on every error P, N and the outputs are left untouched:
+ *   OVB_ERR_ARG       ranges that overlap or fall outside N (landmarks and marginalized ranges alike), a landmark both
+ *                     re-anchored and marginalized, a global representation, an anchor camera or clone outside the frame,
+ *                     a new anchor clone or an anchor's extrinsics that is being marginalized, an anchor variable that
+ *                     overlaps a re-anchored landmark; and a singular H_f in the new anchor (ovb_slam_anchor_change
+ *                     reports the same; for the device-computed representations it is found on the device, after the
+ *                     upload, and the kernels that would read the landmark's Phi do nothing);
+ *   OVB_ERR_NEG_DIAG  a propagated landmark diagonal is negative. ovb_cov_propagate writes P before it reports this; this call
+ *                     does not;
+ *   OVB_ERR_CAPACITY  the call's inputs (frame, landmark records, index maps, Phi slots) exceed the staging the context
+ *                     reserved at ovb_create (max_rows / max_meas and max_state size it);
+ *   OVB_ERR_CUDA      a CUDA runtime error (ovb_last_error).
+ * One H2D copy (frame and anchor list), one D2H copy (new values and status) and one stream synchronisation. */
+ovb_status ovb_marginalize_window(ovb_ctx *ctx, const ovb_frame *frame, const ovb_opts *opts, const int32_t *marg_off, const int32_t *marg_sz,
+                                  int n_marg, const ovb_anchor_changes *anchors);
+
 /* StateHelper::EKFUpdate with R = sigma2·I (UpdaterMSCKF.cpp:282) or R = diag(Rdiag) (UpdaterSLAM.cpp:444).
  * H is r×n row-major, n = Σ sz.                                                   state/StateHelper.cpp:116-197 */
 ovb_status ovb_ekf_update(ovb_ctx *ctx, const int *off, const int *sz, int nvar, const double *H, int r, const double *res,

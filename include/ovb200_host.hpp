@@ -644,5 +644,109 @@ private:
   FeatureInitializerOptions _init;
 };
 
+// The end of VioManager::do_feature_propagate_update as one ovb_marginalize_window: StateHelper::marginalize_slam (the
+// landmarks with should_marg and a featid above 4 * max_aruco_features), then, when the window is full,
+// UpdaterSLAM::change_anchors (every anchored landmark of the oldest clone moves to the newest clone, same camera) and
+// StateHelper::marginalize_old_clone. The landmarks' values and anchors and every id afterwards are those of the three steps
+// called one after the other; the covariance is bit-identical to theirs when it is symmetric, as the filter keeps it (the
+// lost landmarks are then removed with the oldest clone, after the anchor changes: include/ovb200.h says why that order
+// changes no bit). `updater` is the UpdaterSLAM whose change_anchors
+// this replaces (it holds no state the step reads).
+inline void marginalize_window(State &state, UpdaterSLAM &updater) {
+  (void)updater;
+  std::vector<Var> marg;
+  std::vector<size_t> lost;
+  for (auto &f : state._features_SLAM)
+    if (f.second->should_marg && (int)f.first > 4 * state._options.max_aruco_features) {
+      marg.push_back(Var(f.second->id, f.second->size()));
+      lost.push_back(f.first);
+    }
+  const bool full = (int)state._clones_IMU.size() > state._options.max_clone_size;
+  const int C = (int)state._clones_IMU.size(), K = (int)state._cameras.size();
+  std::vector<double> cR((size_t)9 * C), cp((size_t)3 * C), cRf((size_t)9 * C), cpf((size_t)3 * C), kR((size_t)9 * K), kp((size_t)3 * K), kin((size_t)8 * K);
+  std::vector<int> coff((size_t)C), kmodel((size_t)K), kext((size_t)K), kintr((size_t)K, -1);
+  int ci = 0;
+  for (const auto &cl : state._clones_IMU) {
+    std::copy(cl.second->Rot, cl.second->Rot + 9, cR.begin() + 9 * ci);
+    std::copy(cl.second->pos, cl.second->pos + 3, cp.begin() + 3 * ci);
+    std::copy(cl.second->Rot_fej, cl.second->Rot_fej + 9, cRf.begin() + 9 * ci);
+    std::copy(cl.second->pos_fej, cl.second->pos_fej + 3, cpf.begin() + 3 * ci);
+    coff[(size_t)ci++] = cl.second->id;
+  }
+  for (int k = 0; k < K; k++) {
+    const Camera &cam = state._cameras[(size_t)k];
+    std::copy(cam.R_ItoC, cam.R_ItoC + 9, kR.begin() + 9 * k);
+    std::copy(cam.p_IinC, cam.p_IinC + 3, kp.begin() + 3 * k);
+    std::copy(cam.intrinsics, cam.intrinsics + 8, kin.begin() + 8 * k);
+    kmodel[(size_t)k] = cam.model;
+    kext[(size_t)k] = state._options.do_calib_camera_pose ? cam.calib_id : -1;
+  }
+  ovb_frame frame{C, K, cR.data(), cp.data(), cRf.data(), cpf.data(), coff.data(), kR.data(), kp.data(), kin.data(), kmodel.data(), kext.data(), kintr.data()};
+  // the landmarks change_anchors would move, in its visiting order; a lost landmark is gone before it runs
+  std::vector<Landmark *> moved;
+  std::vector<int32_t> lm_off, reps, ocam, oclone, ncam, nclone;
+  std::vector<double> val, val_fej;
+  if (full) {
+    const double marg_timestep = state._clones_IMU.begin()->first;
+    for (auto &f : state._features_SLAM) {
+      Landmark &lm = *f.second;
+      if (lm._feat_representation == OVB_REP_GLOBAL_3D || lm._feat_representation == OVB_REP_GLOBAL_FULL_INVERSE_DEPTH ||
+          lm._anchor_clone_timestamp != marg_timestep || std::find(lost.begin(), lost.end(), f.first) != lost.end())
+        continue;
+      moved.push_back(&lm);
+      lm_off.push_back(lm.id);
+      reps.push_back(lm._feat_representation);
+      ocam.push_back(lm._anchor_cam_id);
+      oclone.push_back(0);
+      ncam.push_back(lm._anchor_cam_id);
+      nclone.push_back(C - 1);
+      val.insert(val.end(), lm.xyz, lm.xyz + 3);
+      val_fej.insert(val_fej.end(), lm.xyz_fej, lm.xyz_fej + 3);
+    }
+    marg.push_back(Var(state._clones_IMU.begin()->second->id, state._clones_IMU.begin()->second->size()));
+  }
+  const int n = (int)moved.size();
+  std::vector<double> nv((size_t)3 * n), nvf((size_t)3 * n);
+  ovb_anchor_changes an{n, lm_off.data(), reps.data(), val.data(), val_fej.data(), ocam.data(), oclone.data(), ncam.data(), nclone.data(), nv.data(), nvf.data()};
+  ovb_opts o;
+  ovb_opts_default(&o);
+  o.do_fej = state._options.do_fej;
+  o.do_calib_camera_pose = state._options.do_calib_camera_pose;
+  std::vector<int32_t> moff, msz;
+  for (const Var &v : marg) {
+    moff.push_back(v.first);
+    msz.push_back(v.second);
+  }
+  if (marg.empty())
+    return;
+  state.check(ovb_marginalize_window(state.ctx(), &frame, &o, moff.data(), msz.data(), (int)marg.size(), n ? &an : nullptr), "marginalize_window");
+  const double new_timestep = state._clones_IMU.rbegin()->first;
+  for (int l = 0; l < n; l++) {
+    std::copy(nv.begin() + 3 * l, nv.begin() + 3 * l + 3, moved[(size_t)l]->xyz);
+    std::copy(nvf.begin() + 3 * l, nvf.begin() + 3 * l + 3, moved[(size_t)l]->xyz_fej);
+    moved[(size_t)l]->_anchor_clone_timestamp = new_timestep;
+  }
+  for (size_t id : lost)
+    state._features_SLAM.erase(id);
+  if (full)
+    state._clones_IMU.erase(state._clones_IMU.begin());
+  // every variable moves up by the sizes of the removed blocks in front of it (StateHelper.cpp:318-326, once per block)
+  auto shift = [&](int &id) {
+    int d = 0;
+    for (const Var &v : marg)
+      if (id > v.first)
+        d += v.second;
+    id -= d;
+  };
+  for (auto &c : state._clones_IMU)
+    shift(c.second->id);
+  for (auto &cam : state._cameras) {
+    shift(cam.calib_id);
+    shift(cam.intrinsics_id);
+  }
+  for (auto &lm : state._features_SLAM)
+    shift(lm.second->id);
+}
+
 } // namespace ovb200
 #endif // OVB200_HOST_HPP

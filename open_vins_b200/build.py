@@ -26,7 +26,7 @@ UNITS = [
     ("k_cholqr.cu", []),
     ("k_ekf.cu", []),
     ("ovb_api.cu", []),
-    ("anchor_change.cu", []),  # host-only math (UpdaterSLAM::perform_anchor_change)
+    ("anchor_change.cu", ["-fmad=false"]),  # UpdaterSLAM::perform_anchor_change, one source for the host and the device
 ]
 HEADERS = ["ovb_internal.cuh", "geom.cuh", "chol.cuh", "chol_tiles.cuh", "chi2_table.inc", os.path.join("..", "..", "include", "ovb200.h")]
 

@@ -203,6 +203,35 @@ class LandmarkArrays:
                              _ptr(self.chi2_multipler, c_double_p))
 
 
+class ovb_anchor_changes(C.Structure):
+    _fields_ = [("n", C.c_int), ("lm_off", c_int_p), ("feat_rep", c_int_p), ("value", c_double_p), ("value_fej", c_double_p),
+                ("old_cam", c_int_p), ("old_clone", c_int_p), ("new_cam", c_int_p), ("new_clone", c_int_p),
+                ("new_value", c_double_p), ("new_value_fej", c_double_p)]
+
+
+class AnchorChanges:
+    """Owns the arrays behind an ovb_anchor_changes: the landmarks ovb_marginalize_window re-anchors, in order. new_value /
+    new_value_fej are written by the call."""
+
+    def __init__(self, lm_off, feat_rep, value, value_fej, old_cam, old_clone, new_cam, new_clone):
+        n = len(lm_off)
+        i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32).reshape(n)
+        self.lm_off, self.feat_rep = i32(lm_off), i32(feat_rep)
+        self.value = np.ascontiguousarray(value, dtype=np.float64).reshape(n, 3)
+        self.value_fej = np.ascontiguousarray(value_fej, dtype=np.float64).reshape(n, 3)
+        self.old_cam, self.old_clone, self.new_cam, self.new_clone = i32(old_cam), i32(old_clone), i32(new_cam), i32(new_clone)
+        self.new_value = np.full((n, 3), np.nan)
+        self.new_value_fej = np.full((n, 3), np.nan)
+
+    def struct(self) -> ovb_anchor_changes:
+        if getattr(self, "_st", None) is None:  # new_value / new_value_fej are written in place: the pointers stay valid
+            self._st = ovb_anchor_changes(len(self.lm_off), _ptr(self.lm_off, c_int_p), _ptr(self.feat_rep, c_int_p), _ptr(self.value, c_double_p),
+                                          _ptr(self.value_fej, c_double_p), _ptr(self.old_cam, c_int_p), _ptr(self.old_clone, c_int_p),
+                                          _ptr(self.new_cam, c_int_p), _ptr(self.new_clone, c_int_p), _ptr(self.new_value, c_double_p),
+                                          _ptr(self.new_value_fej, c_double_p))
+        return self._st
+
+
 class FeatOut:
     def __init__(self, n_feats: int):
         self.status = np.zeros(n_feats, dtype=np.int32)
@@ -264,6 +293,7 @@ def load_library(path: str | None = None) -> C.CDLL:
                                        C.c_double, c_int_p, c_double_p, c_double_p]
     lib.ovb_slam_anchor_change.argtypes = [C.POINTER(ovb_frame), C.POINTER(ovb_opts), C.c_int, c_double_p, c_double_p, C.c_int, C.c_int, C.c_int,
                                            C.c_int, c_double_p, c_double_p, c_double_p, c_int_p, c_int_p, c_int_p, c_int_p]
+    lib.ovb_marginalize_window.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_opts), c_int_p, c_int_p, C.c_int, C.POINTER(ovb_anchor_changes)]
     lib.ovb_slam_update.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_landmarks), C.POINTER(ovb_opts),
                                     C.POINTER(ovb_feat_out), c_double_p, C.POINTER(ovb_stats)]
     lib.ovb_slam_delayed_init.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts), c_double_p, c_double_p, INIT_CALLBACK,
@@ -307,7 +337,7 @@ EXPORTED_SYMBOLS = [
     "ovb_create", "ovb_destroy", "ovb_last_error", "ovb_abi_version", "ovb_opts_default", "ovb_cov_set", "ovb_cov_get",
     "ovb_cov_dim", "ovb_cov_get_marginal", "ovb_cov_clone", "ovb_cov_marginalize", "ovb_cov_propagate", "ovb_cov_propagate_imu", "ovb_cov_initialize",
     "ovb_msckf_update", "ovb_slam_update", "ovb_slam_update_reps", "ovb_set_slam_unbounded", "ovb_slam_delayed_init", "ovb_slam_delayed_init_reps",
-    "ovb_slam_anchor_change", "ovb_ekf_update", "ovb_triangulate", "ovb_feature_jacobians", "ovb_compress", "ovb_compress_gram", "ovb_compress_cholqr2",
+    "ovb_slam_anchor_change", "ovb_marginalize_window", "ovb_ekf_update", "ovb_triangulate", "ovb_feature_jacobians", "ovb_compress", "ovb_compress_gram", "ovb_compress_cholqr2",
     "ovb_chi2_quantile95", "ovb_last_stage_ms", "ovb_set_replay", "ovb_msckf_replay", "ovb_last_counters", "ovb_last_init_counters", "ovb_last_host_us", "ovb_set_profile", "ovb_profile_read",
     "ovb_set_stream", "ovb_msckf_shard_compress", "ovb_msckf_shard_compress_range", "ovb_shard_partition", "ovb_msckf_shard_finish",
 ]
@@ -407,6 +437,16 @@ class Engine:
 
     def cov_marginalize(self, off, size):
         self._check(self.lib.ovb_cov_marginalize(self.h, off, size))
+
+    def marginalize_window(self, frame, opts, marg_off, marg_sz, anchors=None):
+        """ovb_marginalize_window: frame is a FrameArrays (or None without anchors), anchors an AnchorChanges (or None).
+        Returns the status (OVB_OK or OVB_ERR_NEG_DIAG; other errors raise); the new values land in anchors."""
+        marg_off = np.ascontiguousarray(marg_off, dtype=np.int32)
+        marg_sz = np.ascontiguousarray(marg_sz, dtype=np.int32)
+        fs = None if frame is None else C.byref(frame.struct())
+        an = None if anchors is None else C.byref(anchors.struct())
+        return self._check(self.lib.ovb_marginalize_window(self.h, fs, None if opts is None else C.byref(opts), _ptr(marg_off, c_int_p),
+                                                           _ptr(marg_sz, c_int_p), len(marg_off), an), allow=(OVB_ERR_NEG_DIAG,))
 
     def cov_propagate(self, new_off, Phi, Q, old_off, old_sz):
         Phi = np.ascontiguousarray(Phi, dtype=np.float64)

@@ -689,15 +689,26 @@ void launch_cov_marginalize(ovb_ctx *ctx, int off, int size) {
 // EKFPropagation (StateHelper.cpp:80-100). old_idx[k] = covariance index of Phi's column k (q of them).
 //  C[a][j]   = sum_k P[a][old_idx[k]] Phi[j][k]                       (Cov_PhiT, N x p)  -> Cbuf
 //  PCP[i][j] = Qsym[i][j] + sum_k Phi[i][k] C[old_idx[k]][j]          (p x p)            -> Sbuf
+// The two per-entry expressions are shared with ovb_marginalize_window's kernels below, which must give the same bits.
+__device__ __forceinline__ double prop_C_entry(const double *P, int ld, int a, int j, int q, const int *old_idx, const double *Phi) {
+  double acc = 0.0;
+  for (int k = 0; k < q; k++)
+    acc += P[(size_t)a * ld + old_idx[k]] * Phi[(size_t)j * q + k];
+  return acc;
+}
+// C[x][j] at C[x * sx + j * sj]
+__device__ __forceinline__ double prop_PCP_entry(double acc, int i, int j, int q, const int *old_idx, const double *Phi, const double *C, size_t sx,
+                                                 size_t sj) {
+  for (int k = 0; k < q; k++)
+    acc += Phi[(size_t)i * q + k] * C[(size_t)old_idx[k] * sx + (size_t)j * sj];
+  return acc;
+}
 __global__ void k_prop_C(const double *P, int ld, int N, int p, int q, const int *old_idx, const double *Phi, double *Cbuf, int ldC) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= N * p)
     return;
   int a = idx / p, j = idx % p;
-  double acc = 0.0;
-  for (int k = 0; k < q; k++)
-    acc += P[(size_t)a * ld + old_idx[k]] * Phi[(size_t)j * q + k];
-  Cbuf[(size_t)a * ldC + j] = acc;
+  Cbuf[(size_t)a * ldC + j] = prop_C_entry(P, ld, a, j, q, old_idx, Phi);
 }
 __global__ void k_prop_PCP(const double *Cbuf, int ldC, int p, int q, const int *old_idx, const double *Phi, const double *Q, double *Sbuf,
                            int ldS) {
@@ -706,9 +717,7 @@ __global__ void k_prop_PCP(const double *Cbuf, int ldC, int p, int q, const int 
     return;
   int i = idx / p, j = idx % p;
   double acc = (i <= j) ? Q[(size_t)i * p + j] : Q[(size_t)j * p + i];
-  for (int k = 0; k < q; k++)
-    acc += Phi[(size_t)i * q + k] * Cbuf[(size_t)old_idx[k] * ldC + j];
-  Sbuf[(size_t)i * ldS + j] = acc;
+  Sbuf[(size_t)i * ldS + j] = prop_PCP_entry(acc, i, j, q, old_idx, Phi, Cbuf, ldC, 1);
 }
 __global__ void k_prop_write(double *P, int ld, int N, int new_off, int p, const double *Cbuf, int ldC, const double *Sbuf, int ldS,
                              DevUpdateInfo *info) {
@@ -735,6 +744,83 @@ void launch_cov_propagate(ovb_ctx *ctx, int new_off, int p, int q, const int *ol
   k_prop_C<<<(N * p + 255) / 256, 256, 0, ctx->stream>>>(P, ld, N, p, q, old_idx_dev, Phi_dev, ctx->d_M, ld);
   k_prop_PCP<<<(p * p + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_M, ld, p, q, old_idx_dev, Phi_dev, Q_dev, ctx->d_S, ld);
   k_prop_write<<<(N * p + 255) / 256, 256, 0, ctx->stream>>>(P, ld, N, new_off, p, ctx->d_M, ld, ctx->d_S, ld, ctx->d_info);
+}
+
+// ovb_marginalize_window: the anchor changes of landmarks l = 0..n-1 (in call order) as one T P T', then the marginalized
+// ranges dropped, with the bits of the sequence  for l: EKFPropagation(l, Phi_l, Q = 0);  marginalize each range, highest
+// first. Writing P' for P after the propagations and u for a moved row (landmark l, row j < p_l), the sequence gives
+//   P'[u][a] = P'[a][u] = C_l[a][j]       for a outside every moved landmark (C_l as k_prop_C computes it on the prior P:
+//                                           a's row and the columns Phi_l reads are untouched by the landmarks before l)
+//   P'[u][v]             = S_l[j][r]       for v = (l, r): k_prop_PCP with Q = 0, from the same C_l
+//   P'[u][v] = P'[v][u]  = C_L[e][jL]      for landmarks E < L, e the row of E, jL the row of L: k_prop_C at L's step reads
+//                                           E's already-moved row, which is C_E over the columns Phi_L reads (L's own
+//                                           columns included: at E's step L's rows were the prior's)
+// Phase 1 (k_win_rows) writes R[u][a] = C_l[a][j] for every a; phase 2 (k_win_blocks) the K x K blocks from R.
+__global__ void k_win_rows(int K, int N, const DevWinLM *__restrict__ lms, const int *__restrict__ row_lm, const double *__restrict__ phi,
+                           const int *__restrict__ idx, const int *__restrict__ q, const double *__restrict__ P, int ld, double *__restrict__ R,
+                           int ldR, const int *flags) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= K * N || flags[1] != 0) // a singular H_f left this landmark without Phi
+    return;
+  const int u = t / N, a = t % N, l = row_lm[u];
+  R[(size_t)u * ldR + a] = prop_C_entry(P, ld, a, u - lms[l].row0, q[l], idx + OVB_WIN_Q * l, phi + (size_t)OVB_WIN_PHI * l);
+}
+__global__ void k_win_blocks(int K, const DevWinLM *__restrict__ lms, const int *__restrict__ row_lm, const double *__restrict__ phi,
+                             const int *__restrict__ idx, const int *__restrict__ q, const double *__restrict__ R, int ldR, double *__restrict__ B,
+                             int *flags) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= K * K || flags[1] != 0)
+    return;
+  const int u = t / K, v = t % K, lu = row_lm[u], lv = row_lm[v];
+  double val;
+  if (lu == lv) {
+    const DevWinLM &lm = lms[lu];
+    const int i = u - lm.row0, j = v - lm.row0;
+    val = prop_PCP_entry(0.0, i, j, q[lu], idx + OVB_WIN_Q * lu, phi + (size_t)OVB_WIN_PHI * lu, R + (size_t)lm.row0 * ldR, 1, ldR);
+    if (i == j && val < 0.0)
+      atomicMin(&flags[0], lm.lm_off + i);
+  } else {
+    const int L = lu > lv ? lu : lv, ue = lu > lv ? v : u, uL = lu > lv ? u : v;
+    val = prop_C_entry(R, ldR, ue, uL - lms[L].row0, q[L], idx + OVB_WIN_Q * L, phi + (size_t)OVB_WIN_PHI * L);
+  }
+  B[(size_t)u * K + v] = val;
+}
+// StateHelper::marginalize of every range at once (k_cov_marg composed from the highest range down): output (i, j) comes
+// from prior indices (src[i], src[j]); it is read transposed when it lies below the diagonal with at least one removed
+// range between its row and its column (exactly one of the sequential steps transposes it then). mv[x] = the moved row
+// of prior index x, or -1. flags set: nothing is written.
+__global__ void k_win_compact(const double *__restrict__ Pin, double *__restrict__ Pout, int ld, int N2, const int *__restrict__ src,
+                              const int *__restrict__ mv, const double *__restrict__ R, int ldR, const double *__restrict__ B, int K,
+                              const int *__restrict__ flags) {
+  const int i = blockIdx.y * blockDim.y + threadIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N2 || j >= N2 || flags[0] != 0x7fffffff || flags[1] != 0)
+    return;
+  const int si = src[i], sj = src[j];
+  const bool tr = i > j && si - sj != i - j;
+  const int x = tr ? sj : si, y = tr ? si : sj;
+  const int ux = mv[x], uy = mv[y];
+  double v;
+  if (ux >= 0 && uy >= 0)
+    v = B[(size_t)ux * K + uy];
+  else if (ux >= 0)
+    v = R[(size_t)ux * ldR + y];
+  else if (uy >= 0)
+    v = R[(size_t)uy * ldR + x];
+  else
+    v = Pin[(size_t)x * ld + y];
+  Pout[(size_t)i * ld + j] = v;
+}
+
+void launch_window_shift(ovb_ctx *ctx, int n, int K, int N2, const DevWinLM *lms, const int *row_lm, const double *phi, const int *idx,
+                         const int *q, const int *src, const int *mv, int *flags, double *R, int ldR, double *B) {
+  const double *P = ctx->P[ctx->cur];
+  const int N = ctx->N, ld = ctx->ldP;
+  if (n > 0) {
+    k_win_rows<<<(K * N + 255) / 256, 256, 0, ctx->stream>>>(K, N, lms, row_lm, phi, idx, q, P, ld, R, ldR, flags);
+    k_win_blocks<<<(K * K + 255) / 256, 256, 0, ctx->stream>>>(K, lms, row_lm, phi, idx, q, R, ldR, B, flags);
+  }
+  dim3 b(32, 8), g((N2 + 31) / 32, (N2 + 7) / 8);
+  k_win_compact<<<g, b, 0, ctx->stream>>>(P, ctx->P[ctx->cur ^ 1], ld, N2, src, mv, R, ldR, B, K, flags);
 }
 
 // Propagator::propagate_and_clone's accumulation over the IMU steps (Propagator.cpp:83-99, Qd of each step :453-464), in

@@ -309,6 +309,178 @@ ovb_status ovb_cov_marginalize(ovb_ctx *ctx, int off, int size) {
   return OVB_OK;
 }
 
+ovb_status ovb_marginalize_window(ovb_ctx *ctx, const ovb_frame *fr, const ovb_opts *op, const int32_t *marg_off, const int32_t *marg_sz, int n_marg,
+                                  const ovb_anchor_changes *an) {
+  if (!ctx || n_marg < 0 || (n_marg > 0 && (!marg_off || !marg_sz)) || (an && an->n < 0))
+    return OVB_ERR_ARG;
+  const int n = an ? an->n : 0, N = ctx->N;
+  auto fail = [&](const char *msg, int i) {
+    snprintf(ctx->err, sizeof(ctx->err), "ovb_marginalize_window: %s (entry %d)", msg, i);
+    return OVB_ERR_ARG;
+  };
+  if (n > 0 && (!fr || !op || !an->lm_off || !an->feat_rep || !an->value || !an->value_fej || !an->old_cam || !an->old_clone || !an->new_cam ||
+                !an->new_clone || !an->new_value || !an->new_value_fej))
+    return OVB_ERR_ARG;
+  // every range the call touches: the marginalized ones (kind 0) and the re-anchored landmarks (kind 1, entry l)
+  struct Range {
+    int off, sz, kind, entry;
+  };
+  std::vector<Range> rng;
+  int removed = 0;
+  for (int i = 0; i < n_marg; i++) {
+    if (marg_off[i] < 0 || marg_sz[i] < 1 || marg_off[i] + marg_sz[i] > N)
+      return fail("marginalized range outside the covariance", i);
+    rng.push_back({marg_off[i], marg_sz[i], 0, i});
+    removed += marg_sz[i];
+  }
+  const bool ext = n > 0 && op->do_calib_camera_pose != 0;
+  if (n > 0 && (fr->n_clones < 1 || fr->n_clones > OVB_MAX_CLONES || fr->n_cams < 1 || fr->n_cams > OVB_MAX_CAMS || !fr->clone_R || !fr->clone_p ||
+                !fr->clone_off || !fr->cam_R || !fr->cam_p || (ext && !fr->cam_ext_off)))
+    return fail("frame without the arrays the anchor changes read", 0);
+  int K = 0;
+  for (int l = 0; l < n; l++) {
+    const int rep = an->feat_rep[l];
+    if (rep < OVB_REP_ANCHORED_3D || rep > OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE) // global representations have no anchor
+      return fail("representation is not an anchored one", l);
+    const int oc = an->old_cam[l], ocl = an->old_clone[l], nc = an->new_cam[l], ncl = an->new_clone[l];
+    if (oc < 0 || oc >= fr->n_cams || nc < 0 || nc >= fr->n_cams || ocl < 0 || ocl >= fr->n_clones || ncl < 0 || ncl >= fr->n_clones)
+      return fail("anchor camera or clone outside the frame", l);
+    if (ext && (fr->cam_ext_off[oc] < 0 || fr->cam_ext_off[nc] < 0))
+      return fail("do_calib_camera_pose set but the anchor camera has no extrinsics", l);
+    const int p = rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE ? 1 : 3;
+    if (an->lm_off[l] < 0 || an->lm_off[l] + p > N)
+      return fail("landmark outside the covariance", l);
+    rng.push_back({an->lm_off[l], p, 1, l});
+    K += p;
+  }
+  std::sort(rng.begin(), rng.end(), [](const Range &a, const Range &b) { return a.off < b.off; });
+  for (size_t s = 1; s < rng.size(); s++)
+    if (rng[s].off < rng[s - 1].off + rng[s - 1].sz)
+      return fail("overlapping ranges (a landmark re-anchored and marginalized, or listed twice)", rng[s].entry);
+  // the anchor variables Phi reads are none of the moved landmarks, and all but the old anchor clone stay in the state (the
+  // old one is read before the marginalization drops it: re-anchoring the landmarks of the oldest clone is what the call is for)
+  for (int l = 0; l < n; l++) {
+    const int var[4] = {fr->clone_off[an->old_clone[l]], fr->clone_off[an->new_clone[l]], ext ? fr->cam_ext_off[an->old_cam[l]] : -1,
+                        ext ? fr->cam_ext_off[an->new_cam[l]] : -1};
+    for (int v = 0; v < (ext ? 4 : 2); v++) {
+      if (var[v] < 0 || var[v] + 6 > N)
+        return fail("anchor variable outside the covariance", l);
+      for (const Range &r : rng)
+        if (var[v] < r.off + r.sz && r.off < var[v] + 6 && (r.kind == 1 || v > 0))
+          return fail(r.kind == 0 ? "the new anchor clone or an anchor's extrinsics is marginalized" : "a landmark overlaps an anchor variable", l);
+    }
+  }
+  const int N2 = N - removed;
+  if (N2 < 1)
+    return fail("the ranges cover the whole covariance", 0);
+  // one H2D block: [DevWinFrame][DevWinLM n][flags 2 int | new values 6n][src N2 | mv N | row_lm K][q n | column indices n]
+  // [Phi n]. The result block goes back in the one D2H copy. k_anchor_phi fills q, the column indices, Phi and the new
+  // values of a landmark on the device, except for ANCHORED_FULL_INVERSE_DEPTH: its Phi goes through acos / atan2 / sin /
+  // cos, whose last bits differ between CUDA and the C library, so ovb_slam_anchor_change computes it here and it is
+  // uploaded (the upload then runs to the end of the Phi slots; without such a landmark it stops before q).
+  const size_t o_lm = align_up(sizeof(DevWinFrame), 256), o_res = o_lm + align_up(sizeof(DevWinLM) * n, 256);
+  const size_t res_bytes = 4 * sizeof(int) + sizeof(double) * 6 * n, o_map = align_up(o_res + res_bytes, 256);
+  const size_t o_q = align_up(o_map + sizeof(int) * ((size_t)N2 + N + K), 256), o_idx = o_q + sizeof(int) * n;
+  const size_t o_phi = align_up(o_idx + sizeof(int) * OVB_WIN_Q * n, 256), total = o_phi + sizeof(double) * OVB_WIN_PHI * n;
+  if (total > sizeof(double) * ctx->Hs_cap) {
+    snprintf(ctx->err, sizeof(ctx->err), "ovb_marginalize_window: %zu bytes of inputs exceed the reserved staging matrix", total);
+    return OVB_ERR_CAPACITY;
+  }
+  OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  {
+    ovb_status es = ensure_stage(ctx, total / sizeof(double) + 1);
+    if (es != OVB_OK)
+      return es;
+  }
+  unsigned char *h = (unsigned char *)ctx->h_stage, *d = (unsigned char *)ctx->d_Hs;
+  if (n > 0) {
+    DevWinFrame *wf = (DevWinFrame *)h;
+    const int nc = fr->n_clones;
+    memcpy(wf->clone_R, fr->clone_R, sizeof(double) * 9 * nc);
+    memcpy(wf->clone_p, fr->clone_p, sizeof(double) * 3 * nc);
+    memcpy(wf->clone_R_fej, fr->clone_R_fej ? fr->clone_R_fej : fr->clone_R, sizeof(double) * 9 * nc);
+    memcpy(wf->clone_p_fej, fr->clone_p_fej ? fr->clone_p_fej : fr->clone_p, sizeof(double) * 3 * nc);
+    memcpy(wf->cam_R, fr->cam_R, sizeof(double) * 9 * fr->n_cams);
+    memcpy(wf->cam_p, fr->cam_p, sizeof(double) * 3 * fr->n_cams);
+    memcpy(wf->clone_off, fr->clone_off, sizeof(int) * nc);
+    for (int k = 0; k < fr->n_cams; k++)
+      wf->cam_ext_off[k] = fr->cam_ext_off ? fr->cam_ext_off[k] : -1;
+  }
+  DevWinLM *lms = (DevWinLM *)(h + o_lm);
+  int *flags = (int *)(h + o_res), *src = (int *)(h + o_map), *mv = src + N2, *row_lm = mv + N;
+  int *hq = (int *)(h + o_q), *hidx = (int *)(h + o_idx);
+  double *hnewv = (double *)(h + o_res + 4 * sizeof(int)), *hphi = (double *)(h + o_phi);
+  flags[0] = 0x7fffffff; // negative diagonal index
+  flags[1] = 0;          // singular H_f
+  for (int x = 0; x < N; x++)
+    mv[x] = -1;
+  bool host_phi = false;
+  for (int l = 0, row0 = 0; l < n; l++) {
+    DevWinLM &w = lms[l];
+    memcpy(w.value, an->value + 3 * l, sizeof(w.value));
+    memcpy(w.value_fej, an->value_fej + 3 * l, sizeof(w.value_fej));
+    w.lm_off = an->lm_off[l];
+    w.rep = an->feat_rep[l];
+    w.p = w.rep == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE ? 1 : 3;
+    w.row0 = row0;
+    w.old_cam = an->old_cam[l], w.old_clone = an->old_clone[l], w.new_cam = an->new_cam[l], w.new_clone = an->new_clone[l];
+    w.host = w.rep == OVB_REP_ANCHORED_FULL_INVERSE_DEPTH;
+    if (w.host) {
+      ovb_opts ol = *op;
+      ol.feat_rep = w.rep;
+      int32_t order_off[8], order_sz[8], n_order = 0, n_cols = 0;
+      if (ovb_slam_anchor_change(fr, &ol, w.lm_off, w.value, w.value_fej, w.old_cam, w.old_clone, w.new_cam, w.new_clone, hnewv + 6 * l,
+                                 hnewv + 6 * l + 3, hphi + (size_t)OVB_WIN_PHI * l, order_off, order_sz, &n_order, &n_cols) != OVB_OK)
+        return fail("H_f in the new anchor is singular", l);
+      int *ix = hidx + OVB_WIN_Q * l;
+      for (int i = 0, c = 0; i < n_order; i++)
+        for (int k = 0; k < order_sz[i]; k++)
+          ix[c++] = order_off[i] + k;
+      hq[l] = n_cols;
+      host_phi = true;
+    }
+    for (int j = 0; j < w.p; j++) {
+      mv[w.lm_off + j] = row0 + j;
+      row_lm[row0 + j] = l;
+    }
+    row0 += w.p;
+  }
+  for (int x = 0, c = 0, r = 0; x < N; x++) { // rng is sorted: skip the marginalized ranges
+    while (r < (int)rng.size() && (rng[r].kind != 0 || rng[r].off + rng[r].sz <= x))
+      r++;
+    if (r < (int)rng.size() && x >= rng[r].off)
+      continue;
+    src[c++] = x;
+  }
+  const size_t up0 = n > 0 ? 0 : o_res; // without anchors the frame and landmark records are not read
+  const size_t up1 = host_phi ? total : o_q;
+  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(d + up0, h + up0, up1 - up0, cudaMemcpyHostToDevice, ctx->stream));
+  int *flags_d = (int *)(d + o_res), *q_d = (int *)(d + o_q), *idx_d = (int *)(d + o_idx);
+  double *newv_d = (double *)(d + o_res + 4 * sizeof(int)), *phi_d = (double *)(d + o_phi);
+  const DevWinLM *lms_d = (const DevWinLM *)(d + o_lm);
+  if (n > 0)
+    launch_anchor_phi(ctx, (const DevWinFrame *)d, lms_d, n, op->do_fej, ext ? 1 : 0, flags_d, newv_d, phi_d, idx_d, q_d);
+  const int *src_d = (const int *)(d + o_map), *mv_d = src_d + N2, *row_lm_d = mv_d + N;
+  launch_window_shift(ctx, n, K, N2, lms_d, row_lm_d, phi_d, idx_d, q_d, src_d, mv_d, flags_d, ctx->d_M, ctx->ldP, ctx->d_S);
+  OVB_CUDA_CHECK(ctx, cudaGetLastError());
+  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_res, d + o_res, res_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+  if (flags[1] != 0)
+    return fail("H_f in the new anchor is singular", 0);
+  if (flags[0] != 0x7fffffff) {
+    snprintf(ctx->err, sizeof(ctx->err), "ovb_marginalize_window: propagated diagonal at %d is negative; P is unchanged", flags[0]);
+    return OVB_ERR_NEG_DIAG;
+  }
+  const double *newv = (const double *)(h + o_res + 4 * sizeof(int));
+  for (int l = 0; l < n; l++) {
+    memcpy(an->new_value + 3 * l, newv + 6 * l, sizeof(double) * 3);
+    memcpy(an->new_value_fej + 3 * l, newv + 6 * l + 3, sizeof(double) * 3);
+  }
+  ctx->cur ^= 1;
+  ctx->N = N2;
+  return OVB_OK;
+}
+
 ovb_status ovb_cov_propagate(ovb_ctx *ctx, int new_off, int p, const int *old_off, const int *old_sz, int nold, const double *Phi,
                              const double *Q) {
   if (!ctx || !old_off || !old_sz || !Phi || !Q || p < 1 || nold < 1 || new_off < 0 || new_off + p > ctx->N)

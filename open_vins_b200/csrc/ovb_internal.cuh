@@ -116,6 +116,28 @@ struct DevInitSys {
 };
 #define OVB_INIT_HEAD_BYTES (4 * sizeof(int) + 4 * sizeof(double))
 
+// ovb_marginalize_window: the frame slice the anchor changes read (FEJ arrays already substituted when the caller has
+// none) and one record per re-anchored landmark; uploaded with the rest of the call's inputs in one H2D copy
+struct DevWinFrame {
+  double clone_R[OVB_MAX_CLONES][9];
+  double clone_p[OVB_MAX_CLONES][3];
+  double clone_R_fej[OVB_MAX_CLONES][9];
+  double clone_p_fej[OVB_MAX_CLONES][3];
+  double cam_R[OVB_MAX_CAMS][9];
+  double cam_p[OVB_MAX_CAMS][3];
+  int clone_off[OVB_MAX_CLONES];
+  int cam_ext_off[OVB_MAX_CAMS];
+};
+struct DevWinLM {
+  double value[3], value_fej[3];
+  int lm_off, rep, p; // covariance id, ovb_feat_rep, width (3, or 1 for ANCHORED_INVERSE_DEPTH_SINGLE)
+  int row0;           // first of its p rows in the moved-row scratch
+  int old_cam, old_clone, new_cam, new_clone;
+  int host;           // 1: Phi, its column indices, q and the new values were computed on the host and uploaded
+};
+#define OVB_WIN_Q 27                 // widest Phi of an anchor change: 2 clones + 2 extrinsics + the landmark
+#define OVB_WIN_PHI (3 * OVB_WIN_Q)  // its doubles
+
 // packed measurement blob layout (device): [meas_off int32 (F+1)][cam u8 (M)][pad][clone u16 (M)][pad][uv f32 2M][uvn f32 2M][keys u8]
 struct BlobView {
   const uint8_t *cam;
@@ -292,6 +314,13 @@ bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, c
 void launch_cov_clone(ovb_ctx *ctx, int old_off, int size, const double *dnc_dt_dev, int dt_off, const int *neg_diag_dev = nullptr);
 void launch_cov_marginalize(ovb_ctx *ctx, int off, int size);
 void launch_cov_propagate(ovb_ctx *ctx, int new_off, int p, int q, const int *old_idx_dev, const double *Phi_dev, const double *Q_dev);
+// ovb_marginalize_window (anchor_change.cu): Phi, column indices and new values of each re-anchored landmark
+void launch_anchor_phi(ovb_ctx *ctx, const DevWinFrame *wf, const DevWinLM *lms, int n, int do_fej, int ext, int *flags, double *new_values,
+                       double *phi, int *idx, int *q);
+// ovb_marginalize_window (k_ekf.cu): the K moved landmark rows into R [K x N] (ld ldR), their K x K blocks into B, then
+// P[cur] compacted through src / mv into P[cur ^ 1]; flags = {negative diagonal index, singular}: set, P stays untouched
+void launch_window_shift(ovb_ctx *ctx, int n, int K, int N2, const DevWinLM *lms, const int *row_lm, const double *phi, const int *idx,
+                         const int *q, const int *src, const int *mv, int *flags, double *R, int ldR, double *B);
 // Phi, Q (n x n, n <= OVB_PROP_MAX_N) accumulated over `steps` IMU steps, F [steps][n][n], G [steps][n][12], qc [steps][4];
 // false when the launch failed
 bool launch_prop_accumulate(ovb_ctx *ctx, int n, int steps, const double *F_dev, const double *G_dev, const double *qc_dev, double *Phi_dev,
