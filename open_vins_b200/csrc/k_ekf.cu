@@ -399,15 +399,21 @@ __global__ void __launch_bounds__(256) k_ekf_downdate1(double *__restrict__ P, i
   }
 }
 
-__global__ void k_ekf_prep(DevUpdateInfo *info, const int *skip) {
+// resets the failure flags and stages the residual, column n of H's first r rows, in w for the Cholesky kernels
+__global__ void k_ekf_prep(DevUpdateInfo *info, const int *skip, const double *__restrict__ H, int ldH, int r, int n, double *__restrict__ w) {
   OVB_PDL_ENTER();
-  info->neg_diag_index = 0x7fffffff;
-  info->not_spd = (skip && *skip) ? 1 : 0; // a skipped update takes the failed-factor exits of the kernels below
-  info->nonfinite = 0;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < r)
+    w[i] = H[(size_t)i * ldH + n];
+  if (i == 0) {
+    info->neg_diag_index = OVB_NO_NEG_DIAG;
+    info->not_spd = (skip && *skip) ? 1 : 0; // a skipped update takes the failed-factor exits of the kernels below
+    info->nonfinite = 0;
+  }
 }
 
-// H: r x n (row-major, ldHm), r <= n <= N (callers compress first when r > n); column j of H is state column
-// d_info->col_state[j]. Everything is enqueued on the context stream; flags land in d_info.
+// H: r x (n+1) (row-major, ldHm), r <= n <= N (callers compress first when r > n); column j < n of H is state column
+// d_info->col_state[j], column n the residual. Everything is enqueued on the context stream; flags land in d_info.
 // gate_only: stop after the Cholesky — d_w then holds w = L^-1 res (|w|^2 = res' S^-1 res) and P is untouched
 // (the Mahalanobis test of StateHelper::initialize, StateHelper.cpp:458-470).
 void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bool gate_only, double sigma2, const double *Rdiag_dev,
@@ -415,7 +421,7 @@ void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bo
   const int N = ctx->N;
   const int ld = ctx->ldP;
   double *P = ctx->P[ctx->cur];
-  ovb_launch(ctx, k_ekf_prep, dim3(1), dim3(1), (size_t)(0), ctx->d_info, skip_dev);
+  ovb_launch(ctx, k_ekf_prep, dim3(r > 128 ? (r + 127) / 128 : 1), dim3(128), (size_t)(0), ctx->d_info, skip_dev, H, ldHm, r, n, ctx->d_w);
   if (r <= 0 || n <= 0)
     return;
   if (!ctx->attr_done[2]) { // function attributes are per device: one flag per context
@@ -439,7 +445,6 @@ void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bo
   }
   size_t chol_bytes = sizeof(double) * (size_t)(r + 1) * (size_t)(r | 1);
   int use_smem = chol_bytes <= 200 * 1024;
-  // the residual vector is column n of H's row (TSQR output) or a separate buffer: callers stage it in d_w
   double *invdiag = ctx->d_w + ctx->cfg.max_state; // d_w holds 4 x max_state doubles: [w | 1/diag(L) | ...]
   double *Lpk = nullptr; // packed factor for the register solve (only written by the DMMA Cholesky)
   unsigned long long epoch = 0; // nonzero: the factor streams into that solve
@@ -627,7 +632,7 @@ void launch_init_prep(ovb_ctx *ctx, int feat, int k, int n) {
 __global__ void k_cov_clone(double *P, int ld, int N, int old_off, int size, const int *neg_diag) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   int N2 = N + size;
-  if (idx >= N2 * size || (neg_diag && *neg_diag != 0x7fffffff))
+  if (idx >= N2 * size || (neg_diag && *neg_diag != OVB_NO_NEG_DIAG))
     return;
   int i = idx / size, j = idx % size; // element (i, N+j) and its mirror (N+j, i)
   double v;
@@ -643,7 +648,7 @@ __global__ void k_cov_clone(double *P, int ld, int N, int old_off, int size, con
 // augment_clone time-offset term, step 1: P[:, N..N+size) += P[:, dt] dnc'   (StateHelper.cpp:611-612)
 __global__ void k_cov_dt_cols(double *P, int ld, int N2, int new_off, int size, int dt_off, const double *dnc, const int *neg_diag) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= N2 * size || (neg_diag && *neg_diag != 0x7fffffff))
+  if (idx >= N2 * size || (neg_diag && *neg_diag != OVB_NO_NEG_DIAG))
     return;
   int i = idx / size, j = idx % size;
   P[(size_t)i * ld + new_off + j] += P[(size_t)i * ld + dt_off] * dnc[j];
@@ -651,7 +656,7 @@ __global__ void k_cov_dt_cols(double *P, int ld, int N2, int new_off, int size, 
 // step 2: P[N..N+size, :] += dnc P[dt, :]   (StateHelper.cpp:613-614) — reads the row written by step 1
 __global__ void k_cov_dt_rows(double *P, int ld, int N2, int new_off, int size, int dt_off, const double *dnc, const int *neg_diag) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= N2 * size || (neg_diag && *neg_diag != 0x7fffffff))
+  if (idx >= N2 * size || (neg_diag && *neg_diag != OVB_NO_NEG_DIAG))
     return;
   int i = idx / N2, j = idx % N2;
   P[(size_t)(new_off + i) * ld + j] += dnc[i] * P[(size_t)dt_off * ld + j];
@@ -740,7 +745,7 @@ __global__ void k_prop_write(double *P, int ld, int N, int new_off, int p, const
 void launch_cov_propagate(ovb_ctx *ctx, int new_off, int p, int q, const int *old_idx_dev, const double *Phi_dev, const double *Q_dev) {
   double *P = ctx->P[ctx->cur];
   int N = ctx->N, ld = ctx->ldP;
-  ovb_launch(ctx, k_ekf_prep, dim3(1), dim3(1), (size_t)(0), ctx->d_info, (const int *)nullptr);
+  ovb_launch(ctx, k_ekf_prep, dim3(1), dim3(1), (size_t)(0), ctx->d_info, (const int *)nullptr, (const double *)nullptr, 0, 0, 0, (double *)nullptr);
   k_prop_C<<<(N * p + 255) / 256, 256, 0, ctx->stream>>>(P, ld, N, p, q, old_idx_dev, Phi_dev, ctx->d_M, ld);
   k_prop_PCP<<<(p * p + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_M, ld, p, q, old_idx_dev, Phi_dev, Q_dev, ctx->d_S, ld);
   k_prop_write<<<(N * p + 255) / 256, 256, 0, ctx->stream>>>(P, ld, N, new_off, p, ctx->d_M, ld, ctx->d_S, ld, ctx->d_info);
@@ -793,7 +798,7 @@ __global__ void k_win_compact(const double *__restrict__ Pin, double *__restrict
                               const int *__restrict__ mv, const double *__restrict__ R, int ldR, const double *__restrict__ B, int K,
                               const int *__restrict__ flags) {
   const int i = blockIdx.y * blockDim.y + threadIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= N2 || j >= N2 || flags[0] != 0x7fffffff || flags[1] != 0)
+  if (i >= N2 || j >= N2 || flags[0] != OVB_NO_NEG_DIAG || flags[1] != 0)
     return;
   const int si = src[i], sj = src[j];
   const bool tr = i > j && si - sj != i - j;

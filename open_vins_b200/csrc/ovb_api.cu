@@ -410,8 +410,8 @@ ovb_status ovb_marginalize_window(ovb_ctx *ctx, const ovb_frame *fr, const ovb_o
   int *flags = (int *)(h + o_res), *src = (int *)(h + o_map), *mv = src + N2, *row_lm = mv + N;
   int *hq = (int *)(h + o_q), *hidx = (int *)(h + o_idx);
   double *hnewv = (double *)(h + o_res + 4 * sizeof(int)), *hphi = (double *)(h + o_phi);
-  flags[0] = 0x7fffffff; // negative diagonal index
-  flags[1] = 0;          // singular H_f
+  flags[0] = OVB_NO_NEG_DIAG; // negative diagonal index
+  flags[1] = 0;               // singular H_f
   for (int x = 0; x < N; x++)
     mv[x] = -1;
   bool host_phi = false;
@@ -467,7 +467,7 @@ ovb_status ovb_marginalize_window(ovb_ctx *ctx, const ovb_frame *fr, const ovb_o
   OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
   if (flags[1] != 0)
     return fail("H_f in the new anchor is singular", 0);
-  if (flags[0] != 0x7fffffff) {
+  if (flags[0] != OVB_NO_NEG_DIAG) {
     snprintf(ctx->err, sizeof(ctx->err), "ovb_marginalize_window: propagated diagonal at %d is negative; P is unchanged", flags[0]);
     return OVB_ERR_NEG_DIAG;
   }
@@ -517,7 +517,7 @@ ovb_status ovb_cov_propagate(ovb_ctx *ctx, int new_off, int p, const int *old_of
   OVB_CUDA_CHECK(ctx, cudaGetLastError());
   OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_info, ctx->d_info, sizeof(DevUpdateInfo), cudaMemcpyDeviceToHost, ctx->stream));
   OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  if (ctx->h_info->neg_diag_index != 0x7fffffff) {
+  if (ctx->h_info->neg_diag_index != OVB_NO_NEG_DIAG) {
     snprintf(ctx->err, sizeof(ctx->err), "EKFPropagation: diagonal at %d is negative", ctx->h_info->neg_diag_index);
     return OVB_ERR_NEG_DIAG;
   }
@@ -599,7 +599,7 @@ ovb_status ovb_cov_propagate_imu(ovb_ctx *ctx, int n, int steps, const double *F
     memcpy(Phi_out, hs, sizeof(double) * nn);
   if (Q_out)
     memcpy(Q_out, hs + nn, sizeof(double) * nn);
-  if (ctx->h_info->neg_diag_index != 0x7fffffff) {
+  if (ctx->h_info->neg_diag_index != OVB_NO_NEG_DIAG) {
     snprintf(ctx->err, sizeof(ctx->err), "EKFPropagation: diagonal at %d is negative", ctx->h_info->neg_diag_index);
     return OVB_ERR_NEG_DIAG;
   }
@@ -608,12 +608,6 @@ ovb_status ovb_cov_propagate_imu(ovb_ctx *ctx, int n, int steps, const double *F
 }
 
 // ------------------------------------------------------------------------------------------------ marshalling
-struct Packed {
-  int n_feats, n_meas, m_total, ldH, n_all;
-  int n_groups; // SLAM: column groups (ctx->h_grp / d_grp); n_all is then the widest group's column count
-  BlobView bv;
-};
-
 // group tables for n groups; several groups also need the prior's snapshot and the correction accumulator
 static ovb_status ensure_groups(ovb_ctx *ctx, int n) {
   if (n > 1) {
@@ -923,9 +917,6 @@ static ovb_status pack_inputs(ovb_ctx *ctx, const ovb_frame *fr, const ovb_feat_
       }
     }
     d.key1 = (int)nkeys;
-    for (int i = d.m0; i < d.m1; i++)
-      if (fb->cam[i] >= fr->n_cams || fb->clone[i] >= fr->n_clones)
-        return OVB_ERR_ARG;
     d.status = OVB_FEAT_OK;
     d.anchor_cam = d.anchor_clone = -1;
     d.chi2 = NAN;
@@ -1041,6 +1032,50 @@ static void unpack_feats(ovb_ctx *ctx, int F, ovb_feat_out *out) {
         out->p_FinG[3 * f + k] = d.p_FinG[k];
     }
   }
+}
+
+// the status of an EKF update from its read-back failure flags, with the message in ctx->err
+static ovb_status ekf_status(ovb_ctx *ctx, const DevUpdateInfo *inf) {
+  if (inf->not_spd) {
+    snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: innovation covariance not positive definite");
+    return OVB_ERR_NOT_SPD;
+  }
+  if (inf->nonfinite) {
+    snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: non-finite covariance entry");
+    return OVB_ERR_NONFINITE;
+  }
+  if (inf->neg_diag_index != OVB_NO_NEG_DIAG) {
+    snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: diagonal at %d is negative", inf->neg_diag_index);
+    return OVB_ERR_NEG_DIAG;
+  }
+  return OVB_OK;
+}
+
+// the read-back of an update's F features, info and dx (the last two in one copy), enqueued behind its kernels; ev[6]
+// marks its end. The caller synchronises.
+static ovb_status enqueue_readback(ovb_ctx *ctx, int F) {
+  const size_t info_dx = ctx->info_bytes + sizeof(double) * (size_t)ctx->N;
+  OVB_CUDA_CHECK(ctx, cudaGetLastError());
+  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_feat, ctx->d_feat, sizeof(DevFeat) * (size_t)F, cudaMemcpyDeviceToHost, ctx->stream));
+  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_info, ctx->d_info, info_dx, cudaMemcpyDeviceToHost, ctx->stream));
+  ctx->last_d2h_bytes = sizeof(DevFeat) * (size_t)F + info_dx;
+  cudaEventRecord(ctx->ev[6], ctx->stream);
+  return OVB_OK;
+}
+
+// ovb_stats of an MSCKF or SLAM update of F features that handed r rows to the EKF update, from the read-back info. The
+// reference's SLAM update hands every stacked row to EKFUpdate (it never compresses there); the MSCKF update compresses.
+static void fill_stats(const ovb_ctx *ctx, ovb_stats *stats, int F, int r, bool slam) {
+  if (!stats)
+    return;
+  const DevUpdateInfo *inf = ctx->h_info;
+  stats->n_feats_in = F;
+  stats->n_feats_used = inf->n_feats_used;
+  stats->rows_stacked = inf->rows_stacked;
+  stats->cols_stacked = inf->n_used;
+  stats->rows_update = slam ? inf->rows_stacked : std::min(inf->rows_stacked, inf->n_used);
+  stats->neg_diag_index = (r > 0 && inf->neg_diag_index != OVB_NO_NEG_DIAG) ? inf->neg_diag_index : -1;
+  stats->ms_total = ctx->stage_ms[5];
 }
 
 // ------------------------------------------------------------------------------------------------ hot path
@@ -1165,7 +1200,6 @@ static void make_givens(double p, double q, double &gc, double &gs) {
   }
 }
 
-__global__ void k_take_z(const double *R, int ldR, int rows, int col, double *w);
 static int compress_system(ovb_ctx *ctx, int mode, double *A, int m, int n, int ldA, double *Rout, int ldR);
 
 // UpdaterSLAM::delayed_init in one call (see include/ovb200.h). Composition of the staged entry points with the state mean
@@ -1301,7 +1335,6 @@ ovb_status ovb_slam_delayed_init_reps(ovb_ctx *ctx, const ovb_frame *frame, cons
       rr = compress_system(ctx, OVB_COMPRESS_CHOLQR2, ctx->d_Hs + (size_t)d.row0 * pk.ldH, rows, n, pk.ldH, ctx->d_R, pk.ldH);
       Hdev = ctx->d_R;
     }
-    ovb_launch(ctx, k_take_z, dim3((rr + 127) / 128), dim3(128), (size_t)(0), Hdev, pk.ldH, rr, n, ctx->d_w);
     ctx->N = N0 + k;
     launch_ekf_update(ctx, Hdev, pk.ldH, rr, n, false, d.sigma_sq, nullptr, skip);
     ctx->N = N0;
@@ -1329,16 +1362,9 @@ ovb_status ovb_slam_delayed_init_reps(ovb_ctx *ctx, const ovb_frame *frame, cons
       continue;
     }
     ctx->N = N0 + k;
-    if (ctx->h_info->not_spd) {
-      snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: innovation covariance not positive definite");
-      return OVB_ERR_NOT_SPD;
-    }
-    if (ctx->h_info->nonfinite)
-      return OVB_ERR_NONFINITE;
-    if (ctx->h_info->neg_diag_index != 0x7fffffff) {
-      snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: diagonal at %d is negative", ctx->h_info->neg_diag_index);
-      return OVB_ERR_NEG_DIAG;
-    }
+    st = ekf_status(ctx, ctx->h_info);
+    if (st != OVB_OK)
+      return st;
     lm_off_out[f] = N0;
     if (on_init) {
       on_init(user, f, N0, k, hs->dx_new, ctx->h_dx, N0 + k); // the host moves its mean and refreshes the frame arrays
@@ -1356,14 +1382,7 @@ ovb_status ovb_last_init_counters(const ovb_ctx *ctx, int64_t out[4]) {
   return OVB_OK;
 }
 
-// copy column n (the residual z) of the n x (n+1) R into d_w so the Cholesky kernel can append it
-__global__ void k_take_z(const double *R, int ldR, int rows, int col, double *w) {
-  OVB_PDL_ENTER();
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < rows)
-    w[i] = R[(size_t)i * ldR + col];
-}
-// col_state for the canonical layout (used by ovb_compress-less paths): info->col_state[j] = slot_off + k
+// dx = 0 when no row reaches the EKF update
 __global__ void k_fill_zero_dx(double *dx, int N) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < N)
@@ -1373,19 +1392,19 @@ __global__ void k_fill_zero_dx(double *dx, int N) {
 // ---- SLAM batches of several column groups: sequential EKF updates at one linearization point. With the rows whitened
 // (R = I), group g's compressed system [R_g | z_g] is applied to the mean already corrected by the groups before it,
 // z_g <- z_g - R_g dx_acc[cols_g]; the result equals the joint update (tests/test_slam_batches_cpu.py).
-// Copies the group's column map into info (the EKF reads it there) and stages the corrected residual in w.
-__global__ void k_group_take_z(const double *__restrict__ R, int ldR, int rows, int n, const int *__restrict__ col_state,
-                               const double *__restrict__ dx_acc, double *__restrict__ w, DevUpdateInfo *__restrict__ info) {
+// Copies the group's column map into info (the EKF reads it there) and writes the corrected residual over column n of R.
+__global__ void k_group_take_z(double *__restrict__ R, int ldR, int rows, int n, const int *__restrict__ col_state,
+                               const double *__restrict__ dx_acc, DevUpdateInfo *__restrict__ info) {
   OVB_PDL_ENTER();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n)
     info->col_state[i] = col_state[i];
   if (i < rows) {
-    const double *Ri = R + (size_t)i * ldR;
+    double *Ri = R + (size_t)i * ldR;
     double z = Ri[n];
     for (int j = 0; j < n; j++)
       z -= Ri[j] * dx_acc[col_state[j]];
-    w[i] = z;
+    Ri[n] = z;
   }
 }
 // dx_acc += dx of the group; the group's failure flags are kept (the next group's EKF resets them in info)
@@ -1406,7 +1425,7 @@ __global__ void k_group_accumulate(const double *__restrict__ dx, double *__rest
 __global__ void k_group_finish(double *__restrict__ P, int ldP, int N, const double *__restrict__ P_prior, const double *__restrict__ dx_acc,
                                double *__restrict__ dx, DevUpdateInfo *__restrict__ info, const int *__restrict__ flags) {
   OVB_PDL_ENTER();
-  const bool failed = flags[0] || flags[1] || info->neg_diag_index != 0x7fffffff;
+  const bool failed = flags[0] || flags[1] || info->neg_diag_index != OVB_NO_NEG_DIAG;
   const int j = blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y * blockDim.y + threadIdx.y;
   if (i == 0 && j < N)
     dx[j] = failed ? 0.0 : dx_acc[j];
@@ -1433,12 +1452,12 @@ static int compress_system(ovb_ctx *ctx, int mode, double *A, int m, int n, int 
 // ev (optional): ev[1] after triangulation, ev[2] after the per-feature systems, ev[3] after the column map, ev[4] after
 // compression, ev[5] after the EKF update. Returns the row count handed to the EKF update.
 // slam: UpdaterSLAM::update — landmarks come from the state (no triangulation), rows are kept unprojected and whitened;
-// n_groups column groups (ctx->h_grp). Several groups: every gate sees the prior P (the per-feature kernel runs once over
+// pk.n_groups column groups (ctx->h_grp). Several groups: every gate sees the prior P (the per-feature kernel runs once over
 // the batch), then each group is compressed and applied in turn (ev[4] then marks the start of that loop).
 static int enqueue_slam_groups(ovb_ctx *ctx, int n_groups, int ldH);
-static int enqueue_update(ovb_ctx *ctx, int F, BlobView bv, int ldH, int m_total, int n_all, int col_order, cudaEvent_t *ev,
-                          bool slam = false, int n_groups = 1) {
-  const int N = ctx->N;
+static int enqueue_update(ovb_ctx *ctx, const Packed &pk, int col_order, cudaEvent_t *ev, bool slam = false) {
+  const int N = ctx->N, F = pk.n_feats, ldH = pk.ldH, m_total = pk.m_total, n_all = pk.n_all, n_groups = pk.n_groups;
+  const BlobView bv = pk.bv;
   ctx->n_launch = 0;
   ctx->n_launch_tsqr_level = 0;
   ctx->prof_n = 0;
@@ -1495,9 +1514,8 @@ static int enqueue_update(ovb_ctx *ctx, int F, BlobView bv, int ldH, int m_total
   if (ev)
     cudaEventRecord(ev[4], ctx->stream);
   if (r > 0) {
-    ovb_launch(ctx, k_take_z, dim3((r + 127) / 128), dim3(128), (size_t)(0), Rfinal, ldR, r, n_all, ctx->d_w);
     launch_ekf_update(ctx, Rfinal, ldR, r, n_all, false, slam ? 1.0 : ctx->h_opts->sigma_pix_sq, nullptr);
-    ctx->n_launch += 7; // take_z + prep, 2 gemm, chol, trsm, downdate
+    ctx->n_launch += 6; // prep, 2 gemm, chol, trsm, downdate
   } else {
     k_fill_zero_dx<<<(N + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_dx, N);
     ctx->n_launch += 1;
@@ -1521,12 +1539,12 @@ static int enqueue_slam_groups(ovb_ctx *ctx, int n_groups, int ldH) {
       continue;
     const int n = G.n_cols;
     const int r = compress_system(ctx, ctx->h_opts->o.compress, ctx->d_Hs + (size_t)G.row0 * ldH, G.rows, n, ldH, ctx->d_R, ldH);
-    ovb_launch(ctx, k_group_take_z, dim3((n + 127) / 128), dim3(128), (size_t)0, (const double *)ctx->d_R, ldH, r, n,
-               (const int *)ctx->d_grp[g].col_state, (const double *)acc, ctx->d_w, ctx->d_info);
+    ovb_launch(ctx, k_group_take_z, dim3((n + 127) / 128), dim3(128), (size_t)0, ctx->d_R, ldH, r, n, (const int *)ctx->d_grp[g].col_state,
+               (const double *)acc, ctx->d_info);
     launch_ekf_update(ctx, ctx->d_R, ldH, r, n, false, 1.0, nullptr);
     ovb_launch(ctx, k_group_accumulate, dim3((N + 255) / 256), dim3(256), (size_t)0, (const double *)ctx->d_dx, acc, N,
                (const DevUpdateInfo *)ctx->d_info, flags);
-    ctx->n_launch += 8; // take_z, prep, 2 gemm, chol, trsm, downdate, accumulate
+    ctx->n_launch += 8; // group_take_z, prep, 2 gemm, chol, trsm, downdate, accumulate
     r_total += r;
   }
   if (r_total > 0) {
@@ -1639,8 +1657,7 @@ ovb_status ovb_msckf_replay(ovb_ctx *ctx, int steps, int flush_l2, float *ms_per
     cudaMemcpyAsync(ctx->P[ctx->cur], ctx->P_snap, Pbytes, cudaMemcpyDeviceToDevice, ctx->stream);
     cudaEvent_t *ev = &evs[(size_t)s * 6];
     cudaEventRecord(ev[0], ctx->stream);
-    enqueue_update(ctx, ctx->last_n_feats, ctx->last_bv, ctx->last_ldH, ctx->last_m_total, ctx->last_n_all, ctx->last_col_order,
-                   ev);
+    enqueue_update(ctx, ctx->last_pk, ctx->last_col_order, ev);
   }
   OVB_CUDA_CHECK(ctx, cudaGetLastError());
   OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1693,20 +1710,13 @@ ovb_status ovb_msckf_update(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat
     OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->P_snap, ctx->P[ctx->cur], sizeof(double) * (size_t)ctx->ldP * N, cudaMemcpyDeviceToDevice,
                                         ctx->stream));
     ctx->last_pk_valid = 1;
-    ctx->last_n_feats = pk.n_feats;
-    ctx->last_m_total = pk.m_total;
-    ctx->last_ldH = pk.ldH;
-    ctx->last_n_all = pk.n_all;
-    ctx->last_bv = pk.bv;
+    ctx->last_pk = pk;
     ctx->last_col_order = opts->col_order;
   }
-  const int r = enqueue_update(ctx, pk.n_feats, pk.bv, pk.ldH, pk.m_total, pk.n_all, opts->col_order, ctx->ev);
-  OVB_CUDA_CHECK(ctx, cudaGetLastError());
-  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_feat, ctx->d_feat, sizeof(DevFeat) * (size_t)F, cudaMemcpyDeviceToHost, ctx->stream));
-  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_info, ctx->d_info, ctx->info_bytes + sizeof(double) * (size_t)N, cudaMemcpyDeviceToHost,
-                                      ctx->stream)); // info + dx in one copy
-  ctx->last_d2h_bytes = sizeof(DevFeat) * (size_t)F + ctx->info_bytes + sizeof(double) * (size_t)N;
-  cudaEventRecord(ctx->ev[6], ctx->stream);
+  const int r = enqueue_update(ctx, pk, opts->col_order, ctx->ev);
+  st = enqueue_readback(ctx, F);
+  if (st != OVB_OK)
+    return st;
   const auto h2 = std::chrono::steady_clock::now();
   OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
   const auto h3 = std::chrono::steady_clock::now();
@@ -1722,31 +1732,8 @@ ovb_status ovb_msckf_update(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat
   }
   ctx->stage_pending = 1; // the five stage times are read from the events when ovb_last_stage_ms asks for them
   cudaEventElapsedTime(&ctx->stage_ms[5], ctx->ev[0], ctx->ev[6]);
-  const DevUpdateInfo *inf = ctx->h_info;
-  if (stats) {
-    stats->n_feats_in = F;
-    stats->n_feats_used = inf->n_feats_used;
-    stats->rows_stacked = inf->rows_stacked;
-    stats->cols_stacked = inf->n_used;
-    stats->rows_update = std::min(inf->rows_stacked, inf->n_used);
-    stats->neg_diag_index = (r > 0 && inf->neg_diag_index != 0x7fffffff) ? inf->neg_diag_index : -1;
-    stats->ms_total = ctx->stage_ms[5];
-  }
-  if (r > 0) {
-    if (inf->not_spd) {
-      snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: innovation covariance not positive definite");
-      return OVB_ERR_NOT_SPD;
-    }
-    if (inf->nonfinite) {
-      snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: non-finite covariance entry");
-      return OVB_ERR_NONFINITE;
-    }
-    if (inf->neg_diag_index != 0x7fffffff) {
-      snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: diagonal at %d is negative", inf->neg_diag_index);
-      return OVB_ERR_NEG_DIAG;
-    }
-  }
-  return OVB_OK;
+  fill_stats(ctx, stats, F, r, false);
+  return r > 0 ? ekf_status(ctx, ctx->h_info) : OVB_OK;
 }
 
 // UpdaterSLAM::update steps 4-5 (update/UpdaterSLAM.cpp:310-470) on the device: same per-feature kernel in its SLAM mode
@@ -1781,13 +1768,10 @@ ovb_status ovb_slam_update_reps(ovb_ctx *ctx, const ovb_frame *frame, const ovb_
     return st;
   const int F = pk.n_feats;
   ctx->last_pk_valid = 0; // the replay path re-runs MSCKF updates only
-  const int r = enqueue_update(ctx, pk.n_feats, pk.bv, pk.ldH, pk.m_total, pk.n_all, opts->col_order, ctx->ev, true, pk.n_groups);
-  OVB_CUDA_CHECK(ctx, cudaGetLastError());
-  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_feat, ctx->d_feat, sizeof(DevFeat) * (size_t)F, cudaMemcpyDeviceToHost, ctx->stream));
-  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_info, ctx->d_info, ctx->info_bytes + sizeof(double) * (size_t)N, cudaMemcpyDeviceToHost,
-                                      ctx->stream)); // info + dx in one copy
-  ctx->last_d2h_bytes = sizeof(DevFeat) * (size_t)F + ctx->info_bytes + sizeof(double) * (size_t)N;
-  cudaEventRecord(ctx->ev[6], ctx->stream);
+  const int r = enqueue_update(ctx, pk, opts->col_order, ctx->ev, true);
+  st = enqueue_readback(ctx, F);
+  if (st != OVB_OK)
+    return st;
   OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
   if (out) {
     for (int f = 0; f < F; f++) {
@@ -1801,31 +1785,8 @@ ovb_status ovb_slam_update_reps(ovb_ctx *ctx, const ovb_frame *frame, const ovb_
     dx[i] = ctx->h_dx[i];
   ctx->stage_pending = 1; // the five stage times are read from the events when ovb_last_stage_ms asks for them
   cudaEventElapsedTime(&ctx->stage_ms[5], ctx->ev[0], ctx->ev[6]);
-  const DevUpdateInfo *inf = ctx->h_info;
-  if (stats) {
-    stats->n_feats_in = F;
-    stats->n_feats_used = inf->n_feats_used;
-    stats->rows_stacked = inf->rows_stacked;
-    stats->cols_stacked = inf->n_used;
-    stats->rows_update = inf->rows_stacked; // what the reference hands to EKFUpdate (it never compresses here)
-    stats->neg_diag_index = (r > 0 && inf->neg_diag_index != 0x7fffffff) ? inf->neg_diag_index : -1;
-    stats->ms_total = ctx->stage_ms[5];
-  }
-  if (r > 0) {
-    if (inf->not_spd) {
-      snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: innovation covariance not positive definite");
-      return OVB_ERR_NOT_SPD;
-    }
-    if (inf->nonfinite) {
-      snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: non-finite covariance entry");
-      return OVB_ERR_NONFINITE;
-    }
-    if (inf->neg_diag_index != 0x7fffffff) {
-      snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: diagonal at %d is negative", inf->neg_diag_index);
-      return OVB_ERR_NEG_DIAG;
-    }
-  }
-  return OVB_OK;
+  fill_stats(ctx, stats, F, r, true);
+  return r > 0 ? ekf_status(ctx, ctx->h_info) : OVB_OK;
 }
 
 ovb_status ovb_last_stage_ms(const ovb_ctx *ctx, float ms[6]) {
@@ -1931,9 +1892,7 @@ ovb_status ovb_msckf_shard_compress(ovb_ctx *ctx, const ovb_frame *frame, const 
   *ld = pk.ldH;
   if ((size_t)pk.n_all * pk.ldH > (size_t)R_cap_doubles)
     return OVB_ERR_CAPACITY;
-  ctx->last_n_feats = pk.n_feats;
-  ctx->last_n_all = pk.n_all;
-  ctx->last_ldH = pk.ldH;
+  ctx->last_pk = pk;
   ctx->n_launch = 0;
   ctx->n_launch_tsqr_level = 0;
   launch_cam_poses(ctx);
@@ -1954,22 +1913,18 @@ ovb_status ovb_msckf_shard_finish(ovb_ctx *ctx, double *stacked_dev, int n_block
   if (!ctx || !stacked_dev || n_blocks < 1 || !dx || ctx->N < 1)
     return OVB_ERR_ARG;
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-  const int N = ctx->N, n_all = ctx->last_n_all, ld = ctx->last_ldH, F = ctx->last_n_feats;
+  const int N = ctx->N, n_all = ctx->last_pk.n_all, ld = ctx->last_pk.ldH, F = ctx->last_pk.n_feats;
   const double *Rfinal = stacked_dev;
   if (n_blocks > 1) {
     compress_system(ctx, ctx->h_opts->o.compress, stacked_dev, n_blocks * n_all, n_all, ld, ctx->d_R, ld);
     Rfinal = ctx->d_R;
   }
-  ovb_launch(ctx, k_take_z, dim3((n_all + 127) / 128), dim3(128), (size_t)(0), Rfinal, ld, n_all, n_all, ctx->d_w);
   launch_ekf_update(ctx, Rfinal, ld, n_all, n_all, false, ctx->h_opts->sigma_pix_sq, nullptr);
-  ctx->n_launch += 7;
+  ctx->n_launch += 6; // prep, 2 gemm, chol, trsm, downdate
   cudaEventRecord(ctx->ev[5], ctx->stream);
-  OVB_CUDA_CHECK(ctx, cudaGetLastError());
-  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_feat, ctx->d_feat, sizeof(DevFeat) * (size_t)F, cudaMemcpyDeviceToHost, ctx->stream));
-  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_info, ctx->d_info, ctx->info_bytes + sizeof(double) * (size_t)N, cudaMemcpyDeviceToHost,
-                                      ctx->stream)); // info + dx in one copy
-  ctx->last_d2h_bytes = sizeof(DevFeat) * (size_t)F + ctx->info_bytes + sizeof(double) * (size_t)N;
-  cudaEventRecord(ctx->ev[6], ctx->stream);
+  ovb_status st = enqueue_readback(ctx, F);
+  if (st != OVB_OK)
+    return st;
   OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
   unpack_feats(ctx, F, out);
   for (int i = 0; i < N; i++)
@@ -1993,16 +1948,10 @@ ovb_status ovb_msckf_shard_finish(ovb_ctx *ctx, double *stacked_dev, int n_block
     stats->rows_stacked = rows;
     stats->cols_stacked = n_all;
     stats->rows_update = n_all;
-    stats->neg_diag_index = inf->neg_diag_index != 0x7fffffff ? inf->neg_diag_index : -1;
+    stats->neg_diag_index = inf->neg_diag_index != OVB_NO_NEG_DIAG ? inf->neg_diag_index : -1;
     stats->ms_total = ctx->stage_ms[5];
   }
-  if (inf->not_spd)
-    return OVB_ERR_NOT_SPD;
-  if (inf->nonfinite)
-    return OVB_ERR_NONFINITE;
-  if (inf->neg_diag_index != 0x7fffffff)
-    return OVB_ERR_NEG_DIAG;
-  return OVB_OK;
+  return ekf_status(ctx, inf);
 }
 
 // ------------------------------------------------------------------------------------------------ staged dense entry points
@@ -2052,30 +2001,8 @@ static ovb_status stage_dense(ovb_ctx *ctx, const double *H, int m, int n, const
   return OVB_OK;
 }
 
-ovb_status ovb_compress(ovb_ctx *ctx, const double *H, int m, int n, const double *res, double *R_out, double *z_out) {
-  if (!ctx || !H || !res || !R_out || !z_out || m < 1 || n < 1)
-    return OVB_ERR_ARG;
-  if (n + 8 > ctx->cfg.max_state + 8)
-    return OVB_ERR_CAPACITY;
-  OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-  int ld;
-  ovb_status st = stage_dense(ctx, H, m, n, res, nullptr, &ld);
-  if (st != OVB_OK)
-    return st;
-  launch_tsqr(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld);
-  OVB_CUDA_CHECK(ctx, cudaGetLastError());
-  double *hs = ctx->h_stage;
-  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(hs, ctx->d_R, sizeof(double) * (size_t)n * ld, cudaMemcpyDeviceToHost, ctx->stream));
-  OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  for (int i = 0; i < n; i++) {
-    for (int j = 0; j < n; j++)
-      R_out[(size_t)i * n + j] = hs[(size_t)i * ld + j];
-    z_out[i] = hs[(size_t)i * ld + n];
-  }
-  return OVB_OK;
-}
-
-ovb_status ovb_compress_gram(ovb_ctx *ctx, const double *H, int m, int n, const double *res, double *R_out, double *z_out) {
+// [H | res] staged, compressed in `mode` (no fallback to another mode) and [R | z] unpacked
+static ovb_status compress_dense(ovb_ctx *ctx, int mode, const double *H, int m, int n, const double *res, double *R_out, double *z_out) {
   if (!ctx || !H || !res || !R_out || !z_out || m < 1 || n < 1)
     return OVB_ERR_ARG;
   if (n > ctx->cfg.max_state)
@@ -2085,31 +2012,12 @@ ovb_status ovb_compress_gram(ovb_ctx *ctx, const double *H, int m, int n, const 
   ovb_status st = stage_dense(ctx, H, m, n, res, nullptr, &ld);
   if (st != OVB_OK)
     return st;
-  if (launch_compress_gram(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld) < 0)
-    return OVB_ERR_CUDA;
-  OVB_CUDA_CHECK(ctx, cudaGetLastError());
-  double *hs = ctx->h_stage;
-  OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(hs, ctx->d_R, sizeof(double) * (size_t)n * ld, cudaMemcpyDeviceToHost, ctx->stream));
-  OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  for (int i = 0; i < n; i++) {
-    for (int j = 0; j < n; j++)
-      R_out[(size_t)i * n + j] = hs[(size_t)i * ld + j];
-    z_out[i] = hs[(size_t)i * ld + n];
-  }
-  return OVB_OK;
-}
-
-ovb_status ovb_compress_cholqr2(ovb_ctx *ctx, const double *H, int m, int n, const double *res, double *R_out, double *z_out) {
-  if (!ctx || !H || !res || !R_out || !z_out || m < 1 || n < 1)
-    return OVB_ERR_ARG;
-  if (n > ctx->cfg.max_state)
-    return OVB_ERR_CAPACITY;
-  OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-  int ld;
-  ovb_status st = stage_dense(ctx, H, m, n, res, nullptr, &ld);
-  if (st != OVB_OK)
-    return st;
-  if (launch_compress_cholqr2(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld) < 0) {
+  if (mode == OVB_COMPRESS_HOUSEHOLDER_TSQR) {
+    launch_tsqr(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld);
+  } else if (mode == OVB_COMPRESS_NORMAL_EQUATIONS) {
+    if (launch_compress_gram(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld) < 0)
+      return OVB_ERR_CUDA;
+  } else if (launch_compress_cholqr2(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld) < 0) {
     snprintf(ctx->err, sizeof(ctx->err), "ovb_compress_cholqr2: %d columns exceed what this path takes", n);
     return OVB_ERR_CAPACITY;
   }
@@ -2123,6 +2031,18 @@ ovb_status ovb_compress_cholqr2(ovb_ctx *ctx, const double *H, int m, int n, con
     z_out[i] = hs[(size_t)i * ld + n];
   }
   return OVB_OK;
+}
+
+ovb_status ovb_compress(ovb_ctx *ctx, const double *H, int m, int n, const double *res, double *R_out, double *z_out) {
+  return compress_dense(ctx, OVB_COMPRESS_HOUSEHOLDER_TSQR, H, m, n, res, R_out, z_out);
+}
+
+ovb_status ovb_compress_gram(ovb_ctx *ctx, const double *H, int m, int n, const double *res, double *R_out, double *z_out) {
+  return compress_dense(ctx, OVB_COMPRESS_NORMAL_EQUATIONS, H, m, n, res, R_out, z_out);
+}
+
+ovb_status ovb_compress_cholqr2(ovb_ctx *ctx, const double *H, int m, int n, const double *res, double *R_out, double *z_out) {
+  return compress_dense(ctx, OVB_COMPRESS_CHOLQR2, H, m, n, res, R_out, z_out);
 }
 
 ovb_status ovb_ekf_update(ovb_ctx *ctx, const int *off, const int *sz, int nvar, const double *H, int r, const double *res, double sigma2,
@@ -2169,8 +2089,6 @@ ovb_status ovb_ekf_update(ovb_ctx *ctx, const int *off, const int *sz, int nvar,
     rr = compress_system(ctx, OVB_COMPRESS_CHOLQR2, ctx->d_Hs, r, n, ld, ctx->d_R, ld);
     Hdev = ctx->d_R;
   }
-  ovb_launch(ctx, k_take_z, dim3((rr + 127) / 128), dim3(128), (size_t)(0), Hdev, ld, rr, n, ctx->d_w);
-  // k_take_z reads column n: for the uncompressed case that is the staged residual column
   launch_ekf_update(ctx, Hdev, ld, rr, n, false, s2, nullptr);
   OVB_CUDA_CHECK(ctx, cudaGetLastError());
   OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_info, ctx->d_info, sizeof(DevUpdateInfo), cudaMemcpyDeviceToHost, ctx->stream));
@@ -2178,17 +2096,7 @@ ovb_status ovb_ekf_update(ovb_ctx *ctx, const int *off, const int *sz, int nvar,
   OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
   for (int i = 0; i < N; i++)
     dx[i] = ctx->h_dx[i];
-  if (ctx->h_info->not_spd) {
-    snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: innovation covariance not positive definite");
-    return OVB_ERR_NOT_SPD;
-  }
-  if (ctx->h_info->nonfinite)
-    return OVB_ERR_NONFINITE;
-  if (ctx->h_info->neg_diag_index != 0x7fffffff) {
-    snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: diagonal at %d is negative", ctx->h_info->neg_diag_index);
-    return OVB_ERR_NEG_DIAG;
-  }
-  return OVB_OK;
+  return ekf_status(ctx, ctx->h_info);
 }
 
 // StateHelper::initialize on the device-resident covariance. The Givens split of the (tiny) system and the 3x3 inverse are
@@ -2297,9 +2205,9 @@ ovb_status ovb_cov_initialize(ovb_ctx *ctx, const int *off, const int *sz, int n
       Hdev = ctx->d_R;
       rr = n;
     }
-    ovb_launch(ctx, k_take_z, dim3((rr + 127) / 128), dim3(128), (size_t)(0), Hdev, ld, rr, n, ctx->d_w);
     std::vector<double> zh((size_t)rr), wh((size_t)rr);
-    OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(zh.data(), ctx->d_w, sizeof(double) * (size_t)rr, cudaMemcpyDeviceToHost, ctx->stream));
+    OVB_CUDA_CHECK(ctx, cudaMemcpy2DAsync(zh.data(), sizeof(double), Hdev + n, sizeof(double) * ld, sizeof(double), rr, cudaMemcpyDeviceToHost,
+                                          ctx->stream)); // z: column n of Hdev
     launch_ekf_update(ctx, Hdev, ld, rr, n, true, sigma2, nullptr);
     OVB_CUDA_CHECK(ctx, cudaGetLastError());
     OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(wh.data(), ctx->d_w, sizeof(double) * (size_t)rr, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2348,7 +2256,6 @@ ovb_status ovb_cov_initialize(ovb_ctx *ctx, const int *off, const int *sz, int n
     dx[i] = 0.0;
   if (rup > 0) {
     // ---- EKFUpdate with the projected part on the augmented covariance (StateHelper.cpp:476-479)
-    ovb_launch(ctx, k_take_z, dim3((rr + 127) / 128), dim3(128), (size_t)(0), Hdev, ld, rr, n, ctx->d_w);
     launch_ekf_update(ctx, Hdev, ld, rr, n, false, sigma2, nullptr);
     OVB_CUDA_CHECK(ctx, cudaGetLastError());
     OVB_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->h_info, ctx->d_info, sizeof(DevUpdateInfo), cudaMemcpyDeviceToHost, ctx->stream));
@@ -2356,16 +2263,7 @@ ovb_status ovb_cov_initialize(ovb_ctx *ctx, const int *off, const int *sz, int n
     OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     for (int i = 0; i < N + k; i++)
       dx[i] = ctx->h_dx[i];
-    if (ctx->h_info->not_spd) {
-      snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: innovation covariance not positive definite");
-      return OVB_ERR_NOT_SPD;
-    }
-    if (ctx->h_info->nonfinite)
-      return OVB_ERR_NONFINITE;
-    if (ctx->h_info->neg_diag_index != 0x7fffffff) {
-      snprintf(ctx->err, sizeof(ctx->err), "EKFUpdate: diagonal at %d is negative", ctx->h_info->neg_diag_index);
-      return OVB_ERR_NEG_DIAG;
-    }
+    return ekf_status(ctx, ctx->h_info);
   }
   return OVB_OK;
 }

@@ -11,6 +11,7 @@
 #define OVB_CR 256                // TSQR rows per chunk
 #define OVB_PROP_MAX_N 64         // widest IMU block of ovb_cov_propagate_imu (15 + IMU intrinsics is 15, 30 or 39)
 #define OVB_PROP_STEPS_RESERVE 64 // IMU steps per frame the staging of ovb_cov_propagate_imu holds from ovb_create (at n = 39)
+#define OVB_NO_NEG_DIAG 0x7fffffff // negative-diagonal index (DevUpdateInfo, ovb_marginalize_window's flags) when none is negative
 
 // ---- device-resident copy of the slice of State the path reads (uploaded once per update call)
 struct DevFrame {
@@ -91,7 +92,7 @@ struct DevUpdateInfo {
   int order_slot[OVB_MAX_VARS]; // slot id of each variable in stacked order (MSCKF updates)
   int col_state[OVB_MAX_COLS];  // covariance index of each stacked column (order applied)
   int col_canon[OVB_MAX_COLS];  // canonical column each stacked column comes from
-  int neg_diag_index;           // EKF: -1 or first negative diagonal
+  int neg_diag_index;           // EKF: first negative diagonal, or OVB_NO_NEG_DIAG
   int not_spd;                  // EKF: Cholesky pivot failure flag
   int nonfinite;
 };
@@ -145,6 +146,13 @@ struct BlobView {
   const float *uv;
   const float *uvn;
   const uint8_t *keys;
+};
+
+// one packed batch (pack_inputs): the arena's sizes and the device view of its measurement blob
+struct Packed {
+  int n_feats, n_meas, m_total, ldH, n_all;
+  int n_groups; // SLAM: column groups (ctx->h_grp / d_grp); n_all is then the widest group's column count
+  BlobView bv;
 };
 
 struct ovb_ctx {
@@ -215,9 +223,10 @@ struct ovb_ctx {
   mutable int stage_pending; // stage_ms[0..4] of the last update not read back from the events yet (done on demand: each read costs ~1.5 us of host time)
   double host_us[4]; // host wall clock of the last ovb_msckf_update: marshalling + H2D enqueue, kernel enqueue, wait, result unpack
   // replay of the last update on device-resident inputs (bench: `value` leg; see ovb_msckf_replay)
+  // (last_pk also carries the sharded pair's batch from ovb_msckf_shard_compress to ovb_msckf_shard_finish)
   int replay_enabled, last_pk_valid;
-  int last_n_feats, last_m_total, last_ldH, last_n_all, last_col_order;
-  BlobView last_bv;
+  Packed last_pk;
+  int last_col_order;
   double *P_snap;
   void *d_flush;
   // SLAM column groups (grown on demand): the group tables, and for batches of several groups the accumulated state
@@ -299,8 +308,8 @@ bool launch_trsm_rows(ovb_ctx *ctx, double *A, int ldA, int m, int nt, const dou
 // exceeds OVB_MAX_COLS or the leading dimensions are odd
 bool launch_chol_solve_wide(ovb_ctx *ctx, double *S, int ldS, int r, double *w, double *invdiag, double *M, int ldM, int N, bool gate_only);
 void launch_reorder_R(ovb_ctx *ctx, const double *Rin, int n_all, int ldRin, double *Rout, int ldRout);
-// EKF update from an upper-trapezoidal / dense H [r x n] (r <= n) with column->state map in d_info; the residual is staged
-// in d_w. gate_only: stop after the Cholesky factor (d_w then holds w = L^-1 res, P is untouched).
+// EKF update from an upper-trapezoidal / dense H [r x (n+1)] (r <= n) whose column n holds the residual, with the
+// column->state map in d_info. gate_only: stop after the Cholesky factor (d_w then holds w = L^-1 res, P is untouched).
 // skip_dev (optional): a device flag read after the previous kernels; nonzero marks the update failed before it starts
 // (info->not_spd), so P is left untouched and dx = 0
 void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bool gate_only, double sigma2, const double *Rdiag_dev,
