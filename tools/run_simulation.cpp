@@ -5,7 +5,7 @@
 // Usage: <exe> --traj FILE(.txt|.bin) [--cams K] [--clones C] [--msckf M] [--pts P] [--frames F] [--calib 0|1]
 //              [--est OUT.txt] [--timing [OUT.csv]] [--capture FRAME PREFIX] [--integration discrete|rk4|analytical]
 //              [--seed-init S] [--seed-perturb S] [--seed-meas S] [--runs K [--jobs J] [--out-dir DIR]] [--consistency [OUT.txt]]
-//              [--cam-model M[,M...]]
+//              [--cam-model M[,M...]] [--slam M [--slam-in-update U] [--slam-delay S] [--feat-rep-slam NAME] [--slam-log OUT.txt]]
 // Prints one JSON line: frames, ATE (alignment none), mean per-stage host times.
 // --cam-model radtan|equi: the camera model of every camera, or one per camera (a mixed rig, e.g. radtan,equi). Equidistant
 // cameras take the TUM-VI cam0 intrinsics on a 512 x 512 image and the rpng_sim extrinsics of their slot (rpng_sim_cameras
@@ -20,14 +20,23 @@
 // its Simulator, VioManager and backend (with the engine: its own ovb_ctx on device 0), so a run computes the same bits
 // whether it runs alone or beside others. Per run, DIR/est_<seed>.txt and, with --timing, DIR/timing_<seed>.csv. The JSON
 // line then lists every run and the mean / population standard deviation of both ATEs, the wall time and runs/s.
+// --slam M: at most M SLAM landmarks in the state (StateOptions::max_slam_features; 0 = MSCKF only, the default), updated in
+// batches of --slam-in-update U (25), promoted from --slam-delay S seconds after the start (1), every landmark in --feat-rep-slam
+// NAME (GLOBAL_3D; one of the six ovb_feat_rep names). The timing CSV gains the "slam update" and "slam delayed" columns when
+// M > 0; so does the JSON line (and every per_run entry), which gains the SLAM and delayed-init status histograms, the mean and
+// maximum live landmarks, the landmarks initialised and marginalised, the anchor changes and the two SLAM stage times.
+// --slam-log OUT.txt (single run, for tests): what every frame did with the landmarks (write_slam_log).
 #ifdef OVB_SIM_ORACLE
-#include "oracle_backend.hpp"
+#include "oracle_slam_backend.hpp"
 #elif defined(OVB_SIM_HOST_PROPAGATION)
 #include "host_propagation_backend.hpp"
 #else
 #include "../include/ovb200_vio.hpp"
 #endif
 #include <atomic>
+#include <climits>
+#include <cmath>
+#include <cstdlib>
 #include <chrono>
 #include <cstdio>
 #include <cstring>
@@ -44,7 +53,40 @@ struct RunnerOptions {
   int cams = 2, clones = 11, msckf = 10, pts = 250, frames = 0, calib = 1;
   int seed_init = 0, seed_perturb = 0, seed_meas = 0;
   std::vector<int> cam_models; // per camera (--cam-model); empty = all radtan
+  int slam = 0, slam_in_update = 25, feat_rep_slam = OVB_REP_GLOBAL_3D;
+  double slam_delay = 1.0;
 };
+
+static const char *const rep_names[] = {"GLOBAL_3D", "GLOBAL_FULL_INVERSE_DEPTH", "ANCHORED_3D", "ANCHORED_FULL_INVERSE_DEPTH",
+                                        "ANCHORED_MSCKF_INVERSE_DEPTH", "ANCHORED_INVERSE_DEPTH_SINGLE"};
+
+// a whole decimal integer / number, nothing else
+static bool parse_int(const std::string &a, int &v) {
+  char *e = nullptr;
+  const long x = std::strtol(a.c_str(), &e, 10);
+  if (a.empty() || *e || x < INT32_MIN || x > INT32_MAX)
+    return false;
+  v = (int)x;
+  return true;
+}
+static bool parse_double(const std::string &a, double &v) {
+  char *e = nullptr;
+  v = std::strtod(a.c_str(), &e);
+  return !a.empty() && !*e && std::isfinite(v);
+}
+
+#ifndef OVB_SIM_ORACLE
+// the covariance the engine context must hold: the base state, max_clones + 1 clone poses during the update, max_slam landmarks
+// three wide (one for ANCHORED_INVERSE_DEPTH_SINGLE)
+static int state_size_bound(const RunnerOptions &o) {
+  const int base = 15 + (o.calib ? 24 + 1 : 0) + o.cams * (o.calib ? 14 : 0);
+  return base + 6 * (o.clones + 1) + o.slam * (o.feat_rep_slam == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE ? 1 : 3);
+}
+static const int engine_max_state = 640; // ovb_config::max_state of the runner's engine context
+#endif
+
+// the SLAM part of a run's JSON (empty without --slam M, M > 0: such a run prints what a run without the flag prints)
+static std::string slam_json(const RunnerOptions &o, const struct RunSummary &s);
 
 // the JSON field of --cam-model (empty without the flag): , "cam_model": ["radtan", "equi", ...]
 static std::string cam_model_json(const RunnerOptions &o) {
@@ -85,7 +127,56 @@ struct RunSummary {
   double nees_ori = 0, nees_pos = 0; // means over the run's frames (with --consistency)
   size_t map_points = 0;
   long status_hist[9] = {0};
+  long slam_hist[9] = {0}, init_hist[9] = {0}, slam_initialized = 0, slam_marginalized = 0, anchor_changes = 0;
+  double slam_live_mean = 0, ms_slam_update = 0, ms_slam_delayed = 0;
+  int slam_live_max = 0;
 };
+
+static std::string slam_json(const RunnerOptions &o, const RunSummary &s) {
+  if (o.slam <= 0)
+    return "";
+  auto hist = [](const long *h) {
+    std::string r = "[";
+    for (int k = 0; k < 9; k++)
+      r += (k ? ", " : "") + std::to_string(h[k]);
+    return r + "]";
+  };
+  char buf[512];
+  std::snprintf(buf, sizeof(buf), ", \"max_slam\": %d, \"max_slam_in_update\": %d, \"dt_slam_delay\": %.17g, \"feat_rep_slam\": \"%s\", \"mean_slam_live\": %.4f, "
+                "\"max_slam_live\": %d, \"slam_initialized\": %ld, \"slam_marginalized\": %ld, \"anchor_changes\": %ld, \"mean_ms_slam_update\": %.4f, "
+                "\"mean_ms_slam_delayed\": %.4f",
+                o.slam, o.slam_in_update, o.slam_delay, rep_names[o.feat_rep_slam], s.slam_live_mean, s.slam_live_max, s.slam_initialized, s.slam_marginalized,
+                s.anchor_changes, s.ms_slam_update, s.ms_slam_delayed);
+  return std::string(buf) + ", \"slam_status_hist\": " + hist(s.slam_hist) + ", \"init_status_hist\": " + hist(s.init_hist);
+}
+
+// --slam-log: per frame a line "F t since_start N n_clones n_landmarks", then one line per list, each "<tag> featid...": P promoted,
+// M the MSCKF batch, U the SLAM updates, D the delayed initialisations, X the landmarks marginalize_slam removed (as
+// featid:update_fail_count), I the landmarks initialised; then "L featid id size anchor_in_window" per landmark at the frame's
+// end (anchor_in_window -1 for the global representations)
+static void write_slam_log(const std::string &path, const std::vector<SlamFrameRecord> &frames) {
+  FILE *f = std::fopen(path.c_str(), "w");
+  if (!f)
+    return;
+  auto ids = [&](const char *tag, const std::vector<size_t> &v) {
+    std::fprintf(f, "%s", tag);
+    for (size_t id : v)
+      std::fprintf(f, " %zu", id);
+    std::fprintf(f, "\n");
+  };
+  for (const auto &r : frames) {
+    std::fprintf(f, "F %.9f %.9f %d %d %zu\n", r.t, r.since_start, r.N, r.n_clones, r.landmarks.size());
+    ids("P", r.promoted), ids("M", r.msckf), ids("U", r.slam_update), ids("D", r.delayed);
+    std::fprintf(f, "X");
+    for (const auto &x : r.marg_fail_count)
+      std::fprintf(f, " %zu:%d", x.first, x.second);
+    std::fprintf(f, "\n");
+    ids("I", r.initialized);
+    for (const auto &l : r.landmarks)
+      std::fprintf(f, "L %ld %ld %ld %ld\n", l[0], l[1], l[2], l[3]);
+  }
+  std::fclose(f);
+}
 
 #ifdef OVB_SIM_ORACLE
 static const char *const backend_name = "oracle";
@@ -97,7 +188,7 @@ static const char *const backend_name = "engine";
 // consistency = record the consistency samples (written to consistency_path unless it is empty)
 static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<double, 8>> &traj_data, int seed_meas, const std::string &est_path,
                           const std::string &timing_path, bool consistency, const std::string &consistency_path, int capture_frame,
-                          const std::string &capture_prefix) {
+                          const std::string &capture_prefix, const std::string &slam_log_path = "") {
   SimParams sp;
   rpng_sim_cameras(o.cams, sp, o.cam_models);
   sp.use_stereo = o.cams > 1;
@@ -113,11 +204,15 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
       o.calib != 0;
   vo.compress = o.compress == "tsqr" ? OVB_COMPRESS_HOUSEHOLDER_TSQR : (o.compress == "gram" ? OVB_COMPRESS_NORMAL_EQUATIONS : OVB_COMPRESS_CHOLQR2);
   vo.integration_method = o.integration == "discrete" ? INTEGRATION_DISCRETE : (o.integration == "analytical" ? INTEGRATION_ANALYTICAL : INTEGRATION_RK4);
+  vo.max_slam_features = o.slam;
+  vo.max_slam_in_update = o.slam_in_update;
+  vo.dt_slam_delay = o.slam_delay;
+  vo.feat_rep_slam = o.feat_rep_slam;
   Simulator sim(sp, traj_data);
 #ifdef OVB_SIM_ORACLE
-  auto backend = std::make_shared<OracleCov>();
+  auto backend = std::make_shared<OracleSlamCov>();
 #else
-  ovb_config cfg{0, 640, std::max(1024, o.msckf), std::max(1024, o.msckf) * 2 * (o.clones + 1) * o.cams / 2 + 1024, 0};
+  ovb_config cfg{0, engine_max_state, std::max(1024, o.msckf), std::max(1024, o.msckf) * 2 * (o.clones + 1) * o.cams / 2 + 1024, 0};
 #ifdef OVB_SIM_HOST_PROPAGATION
   auto backend = std::make_shared<HostPropagationEngineCov>(cfg);
 #else
@@ -125,6 +220,7 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
 #endif
 #endif
   VioManager sys(vo, sp, backend);
+  sys.record_slam_frames = !slam_log_path.empty();
   if (capture_frame >= 0) {
     // dump the marshalled inputs of ONE update (the golden "update case" wire format of tests/golden_io.py:
     // little-endian, a text header line with the array shapes followed by the raw arrays) and the prior covariance
@@ -180,13 +276,21 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
     sys.write_timing_csv(timing_path);
   if (!consistency_path.empty())
     write_consistency_file(consistency_path, sys.state, res.consistency);
-  double t_prop = 0, t_msckf = 0, t_total = 0, feats = 0, used = 0, rows = 0;
+  if (!slam_log_path.empty())
+    write_slam_log(slam_log_path, sys.slam_frames);
+  double t_prop = 0, t_msckf = 0, t_total = 0, feats = 0, used = 0, rows = 0, t_su = 0, t_sd = 0, live = 0;
+  RunSummary s;
   for (const auto &t : sys.timing) {
     t_prop += t.time_prop, t_msckf += t.time_msckf, t_total += t.time_total;
     feats += t.feats_in, used += t.feats_used, rows += t.rows;
+    t_su += t.time_slam_update, t_sd += t.time_slam_delayed, live += t.slam_live;
+    s.slam_live_max = std::max(s.slam_live_max, t.slam_live);
   }
   const double n = sys.timing.empty() ? 1.0 : (double)sys.timing.size();
-  RunSummary s;
+  s.slam_live_mean = live / n, s.ms_slam_update = 1e3 * t_su / n, s.ms_slam_delayed = 1e3 * t_sd / n;
+  for (int k = 0; k < 9; k++)
+    s.slam_hist[k] = sys.slam_status_hist[k], s.init_hist[k] = sys.init_status_hist[k];
+  s.slam_initialized = sys.slam_initialized, s.slam_marginalized = sys.slam_marginalized, s.anchor_changes = sys.anchor_changes;
   s.feats_in = feats / n, s.feats_used = used / n, s.rows = rows / n;
   s.ms_prop = 1e3 * t_prop / n, s.ms_msckf = 1e3 * t_msckf / n, s.ms_total = 1e3 * t_total / n;
   s.frames = res.frames;
@@ -259,7 +363,7 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
       std::snprintf(buf, sizeof(buf), ", \"nees_ori\": %.17g, \"nees_pos\": %.17g", s.nees_ori, s.nees_pos);
       per_run += buf;
     }
-    per_run += "}";
+    per_run += slam_json(o, s) + "}";
   }
   // the same statistics of the per-run mean NEES
   std::string nees;
@@ -286,7 +390,8 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
 
 int main(int argc, char **argv) {
   RunnerOptions o;
-  std::string est_path, timing_path, consistency_path, capture_prefix, out_dir, cam_model_arg;
+  std::string est_path, timing_path, consistency_path, capture_prefix, out_dir, cam_model_arg, slam_log_path;
+  std::string bad_slam; // the first malformed SLAM option
   int capture_frame = -1, runs = 0, jobs = 0;
   bool timing = false, consistency = false, cam_model = false;
   for (int i = 1; i < argc; i++) {
@@ -320,7 +425,36 @@ int main(int argc, char **argv) {
     else if (a == "--jobs") jobs = std::stoi(next());
     else if (a == "--out-dir") out_dir = next();
     else if (a == "--cam-model") { cam_model = true; cam_model_arg = next(); }
+    else if (a == "--slam") { const std::string v = next(); if (!parse_int(v, o.slam) || o.slam < 0) bad_slam = a + " " + v; }
+    else if (a == "--slam-in-update") { const std::string v = next(); if (!parse_int(v, o.slam_in_update) || o.slam_in_update < 1) bad_slam = a + " " + v; }
+    else if (a == "--slam-delay") { const std::string v = next(); if (!parse_double(v, o.slam_delay) || o.slam_delay < 0) bad_slam = a + " " + v; }
+    else if (a == "--feat-rep-slam") {
+      const std::string v = next();
+      const auto it = std::find(std::begin(rep_names), std::end(rep_names), v);
+      if (it == std::end(rep_names))
+        bad_slam = a + " " + v;
+      else
+        o.feat_rep_slam = (int)(it - std::begin(rep_names));
+    }
+    else if (a == "--slam-log") slam_log_path = next();
   }
+  if (!bad_slam.empty()) {
+    std::fprintf(stderr, "malformed '%s': --slam takes an integer >= 0, --slam-in-update an integer >= 1, --slam-delay seconds >= 0, --feat-rep-slam one of "
+                 "GLOBAL_3D GLOBAL_FULL_INVERSE_DEPTH ANCHORED_3D ANCHORED_FULL_INVERSE_DEPTH ANCHORED_MSCKF_INVERSE_DEPTH ANCHORED_INVERSE_DEPTH_SINGLE\n",
+                 bad_slam.c_str());
+    return 2;
+  }
+  if (runs > 0 && !slam_log_path.empty()) {
+    std::fprintf(stderr, "--slam-log is a single-run option\n");
+    return 2;
+  }
+#ifndef OVB_SIM_ORACLE
+  if (state_size_bound(o) > engine_max_state) {
+    std::fprintf(stderr, "a state of up to %d variables (--cams %d --clones %d --calib %d --slam %d) does not fit the engine context's %d\n", state_size_bound(o),
+                 o.cams, o.clones, o.calib, o.slam, engine_max_state);
+    return 2;
+  }
+#endif
   if (runs < 0 || jobs < 0 || (runs == 0 && (jobs > 0 || !out_dir.empty())) || (runs > 0 && (!est_path.empty() || capture_frame >= 0))) {
     std::fprintf(stderr, "--runs K takes --jobs J >= 1 and --out-dir DIR; --jobs and --out-dir need --runs; --est and --capture are single-run options\n");
     return 2;
@@ -355,7 +489,7 @@ int main(int argc, char **argv) {
     return run_batch(o, traj_data, runs, jobs, out_dir, timing, consistency);
   }
   try {
-    const RunSummary s = run_one(o, traj_data, o.seed_meas, est_path, timing_path, consistency, consistency_path, capture_frame, capture_prefix);
+    const RunSummary s = run_one(o, traj_data, o.seed_meas, est_path, timing_path, consistency, consistency_path, capture_frame, capture_prefix, slam_log_path);
     char nees[128] = "";
     if (consistency)
       std::snprintf(nees, sizeof(nees), ", \"nees_ori\": %.12g, \"nees_pos\": %.12g", s.nees_ori, s.nees_pos);
@@ -364,7 +498,7 @@ int main(int argc, char **argv) {
                 "\"mean_ms_propagation\": %.4f, \"mean_ms_msckf_update\": %.4f, \"mean_ms_total\": %.4f, \"map_points\": %zu, \"status_hist\": [%ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld]%s}\n",
                 backend_name, s.frames, o.cams, cam_model_json(o).c_str(), o.clones, o.msckf, o.pts, o.calib, s.state_dim, s.ate_pos, s.ate_ori_deg, s.feats_in, s.feats_used, s.rows,
                 s.ms_prop, s.ms_msckf, s.ms_total, s.map_points, s.status_hist[0], s.status_hist[1], s.status_hist[2], s.status_hist[3], s.status_hist[4],
-                s.status_hist[5], s.status_hist[6], s.status_hist[7], s.status_hist[8], nees);
+                s.status_hist[5], s.status_hist[6], s.status_hist[7], s.status_hist[8], (nees + slam_json(o, s)).c_str());
   } catch (const std::exception &e) {
     std::fprintf(stderr, "run_simulation failed: %s\n", e.what());
     return 1;
