@@ -1632,8 +1632,8 @@ inline double nees3(const double *A, int lda, const Vec3 &x) {
 }
 
 // one frame: `st` after the update and the clone marginalization, `gt` = Simulator::get_state's [t q p v bg ba] at the
-// frame's IMU time, `truth` = the simulator's configuration (rpng_sim does not perturb the calibration, so the configured
-// value is the true one), P = the base block [0, base_size)^2 of the covariance, row-major
+// frame's IMU time, `truth` = Simulator::get_true_parameters (with sim_do_perturbation the filter starts from a perturbed
+// copy), P = the base block [0, base_size)^2 of the covariance, row-major
 inline ConsistencySample consistency_sample(const VioState &st, const SimParams &truth, const std::array<double, 17> &gt, const std::vector<double> &P) {
   const int n = st.base_size;
   ConsistencySample s;
@@ -1737,7 +1737,8 @@ inline SimRunResult run_simulation(Simulator &sim, VioManager &sys, int max_fram
   std::array<double, 17> imustate;
   if (!sim.get_state(next_imu_time, imustate))
     throw Error(OVB_ERR_ARG, "[SIM]: could not initialize the filter to the first state");
-  imustate[0] -= sim.params.calib_camimu_dt;
+  const SimParams &truth = sim.get_true_parameters();
+  imustate[0] -= truth.calib_camimu_dt;
   sys.initialize_with_gt(imustate);
   double buffer_timecam = -1;
   std::vector<int> buffer_camids;
@@ -1757,7 +1758,7 @@ inline SimRunResult run_simulation(Simulator &sim, VioManager &sys, int max_fram
         if (sys.trajectory_est.size() > before) {
           std::array<double, 17> gt;
           const TrajSample &e = sys.trajectory_est.back();
-          const bool have_gt = sim.get_state(e.t + sim.params.calib_camimu_dt, gt);
+          const bool have_gt = sim.get_state(e.t + truth.calib_camimu_dt, gt);
           if (have_gt)
             res.gt.push_back({e.t, {gt[1], gt[2], gt[3], gt[4]}, {gt[5], gt[6], gt[7]}});
           else
@@ -1767,7 +1768,7 @@ inline SimRunResult run_simulation(Simulator &sim, VioManager &sys, int max_fram
             if (!have_gt) // past the trajectory's end: like the ATE, the estimate stands in for the truth
               gt = {st.timestamp, st.q[0], st.q[1], st.q[2], st.q[3], st.p[0], st.p[1], st.p[2], st.v[0], st.v[1], st.v[2],
                     st.bg[0], st.bg[1], st.bg[2], st.ba[0], st.ba[1], st.ba[2]};
-            res.consistency.push_back(consistency_sample(st, sim.params, gt, sys.cov->get_marginal({0}, {st.base_size})));
+            res.consistency.push_back(consistency_sample(st, truth, gt, sys.cov->get_marginal({0}, {st.base_size})));
           }
         }
         if (max_frames > 0 && sys.frames_done >= max_frames)

@@ -24,7 +24,7 @@ CASE_CONFIG2 = os.path.join(os.path.dirname(HERE), "tests", "golden", "rpng_sim_
 
 def run(exe=None, traj=None, cams=2, clones=11, msckf=10, pts=250, frames=0, calib=1, est=None, timing=None, capture=None, integration="rk4",
         compress="cholqr2", seed_init=0, seed_perturb=0, seed_meas=0, runs=None, jobs=None, out_dir=None, consistency=None, cam_model=None,
-        slam=None, slam_in_update=None, slam_delay=None, feat_rep_slam=None, slam_log=None, timeout=1800):
+        slam=None, slam_in_update=None, slam_delay=None, feat_rep_slam=None, slam_log=None, perturb=False, timeout=1800):
     """Runs the simulation; returns the parsed JSON summary. capture = (frame_index, path_prefix) dumps that update's inputs.
     seed_init / seed_perturb / seed_meas: the simulator's random seeds (rpng_sim's sim_seed_state_init, sim_seed_preturb,
     sim_seed_measurements). runs = K: a Monte-Carlo batch in one process, run r with measurement seed seed_meas + r, on
@@ -37,7 +37,10 @@ def run(exe=None, traj=None, cams=2, clones=11, msckf=10, pts=250, frames=0, cal
     image (INTEGRATION.md §8), and the summary gains "cam_model". None runs the rpng_sim radtan cameras. slam = M: at most M SLAM
     landmarks (--slam), with slam_in_update / slam_delay / feat_rep_slam (a representation name, e.g. "ANCHORED_3D") passed as
     --slam-in-update / --slam-delay / --feat-rep-slam when given; for M > 0 the summary gains the SLAM fields (INTEGRATION.md
-    §8). slam_log = PATH writes the per-frame landmark log (--slam-log, single runs)."""
+    §8). slam_log = PATH writes the per-frame landmark log (--slam-log, single runs). perturb = True starts the filter from a
+    calibration perturbed with seed_perturb (seed_perturb + r for run r of a batch; --perturb, needs calib=1); the summary
+    gains "perturb" and the RMS of err/σ per calibration block at the first and last frame ("calib_nerr_first",
+    "calib_nerr_last"), with their mean and population standard deviation over a batch."""
     cmd = [exe or ENGINE_EXE, "--traj", traj or TRAJ_FIXTURE, "--cams", str(cams), "--clones", str(clones), "--msckf", str(msckf), "--pts", str(pts),
            "--frames", str(frames), "--calib", str(int(calib)), "--integration", integration, "--compress", compress,
            "--seed-init", str(seed_init), "--seed-perturb", str(seed_perturb), "--seed-meas", str(seed_meas)]
@@ -53,6 +56,8 @@ def run(exe=None, traj=None, cams=2, clones=11, msckf=10, pts=250, frames=0, cal
                     ("--slam-log", slam_log)):
         if v is not None:
             cmd += [flag, str(v)]
+    if perturb:
+        cmd += ["--perturb"]
     if capture:
         cmd += ["--capture", str(capture[0]), capture[1]]
     if runs:

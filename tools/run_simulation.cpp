@@ -6,6 +6,7 @@
 //              [--est OUT.txt] [--timing [OUT.csv]] [--capture FRAME PREFIX] [--integration discrete|rk4|analytical]
 //              [--seed-init S] [--seed-perturb S] [--seed-meas S] [--runs K [--jobs J] [--out-dir DIR]] [--consistency [OUT.txt]]
 //              [--cam-model M[,M...]] [--slam M [--slam-in-update U] [--slam-delay S] [--feat-rep-slam NAME] [--slam-log OUT.txt]]
+//              [--perturb]
 // Prints one JSON line: frames, ATE (alignment none), mean per-stage host times.
 // --cam-model radtan|equi: the camera model of every camera, or one per camera (a mixed rig, e.g. radtan,equi). Equidistant
 // cameras take the TUM-VI cam0 intrinsics on a 512 x 512 image and the rpng_sim extrinsics of their slot (rpng_sim_cameras
@@ -26,6 +27,11 @@
 // M > 0; so does the JSON line (and every per_run entry), which gains the SLAM and delayed-init status histograms, the mean and
 // maximum live landmarks, the landmarks initialised and marginalised, the anchor changes and the two SLAM stage times.
 // --slam-log OUT.txt (single run, for tests): what every frame did with the landmarks (write_slam_log).
+// --perturb (rpng_sim's sim_do_perturbation; needs --calib 1): the filter starts from a calibration the simulator perturbs
+// with --seed-perturb (Simulator::perturb_parameters), while the measurements and the truth stay the true ones. With
+// --runs, run r also takes perturbation seed seed_perturb + r. The JSON line (and every per_run entry) gains "perturb" and
+// the RMS of err/σ per calibration block at the first and the last frame (calib_nerr_json); a batch, their mean and
+// population standard deviation over the runs.
 #ifdef OVB_SIM_ORACLE
 #include "oracle_slam_backend.hpp"
 #elif defined(OVB_SIM_HOST_PROPAGATION)
@@ -55,6 +61,7 @@ struct RunnerOptions {
   std::vector<int> cam_models; // per camera (--cam-model); empty = all radtan
   int slam = 0, slam_in_update = 25, feat_rep_slam = OVB_REP_GLOBAL_3D;
   double slam_delay = 1.0;
+  bool perturb = false;
 };
 
 static const char *const rep_names[] = {"GLOBAL_3D", "GLOBAL_FULL_INVERSE_DEPTH", "ANCHORED_3D", "ANCHORED_FULL_INVERSE_DEPTH",
@@ -130,7 +137,50 @@ struct RunSummary {
   long slam_hist[9] = {0}, init_hist[9] = {0}, slam_initialized = 0, slam_marginalized = 0, anchor_changes = 0;
   double slam_live_mean = 0, ms_slam_update = 0, ms_slam_delayed = 0;
   int slam_live_max = 0;
+  double nerr_first[9] = {0}, nerr_last[9] = {0}; // with --perturb: calib_nerr of the first and the last frame
 };
+
+// the calibration blocks of --perturb's report, in calib_nerr's order
+static const char *const calib_blocks[9] = {"dt", "ext_ori", "ext_pos", "intr_fc", "intr_dist", "dw", "da", "tg", "gyro"};
+
+// RMS of err/σ over the coordinates of each calibration block of one consistency sample, pooled over the cameras for the
+// per-camera blocks (every block is in the state: --perturb needs --calib 1)
+static void calib_nerr(const VioState &st, const ConsistencySample &c, double out[9]) {
+  double ss[9] = {0};
+  int n[9] = {0};
+  auto add = [&](int b, int id, int m) {
+    for (int k = id; k < id + m; k++) {
+      const double z = c.err[(size_t)k] / c.sigma[(size_t)k];
+      ss[b] += z * z, n[b]++;
+    }
+  };
+  add(0, st.dt_id, 1);
+  for (const auto &cam : st.cams) {
+    add(1, cam.ext_id, 3), add(2, cam.ext_id + 3, 3);
+    add(3, cam.intr_id, 4), add(4, cam.intr_id + 4, 4);
+  }
+  add(5, st.dw_id, 6), add(6, st.da_id, 6), add(7, st.tg_id, 9), add(8, st.gyro_id, 3);
+  for (int b = 0; b < 9; b++)
+    out[b] = std::sqrt(ss[b] / n[b]);
+}
+
+// {"dt": x, "ext_ori": x, ...} with printf format `fmt` per number
+static std::string blocks_json(const double v[9], const char *fmt) {
+  std::string r = "{";
+  for (int b = 0; b < 9; b++) {
+    char buf[64];
+    std::snprintf(buf, sizeof(buf), fmt, v[b]);
+    r += std::string(b ? ", \"" : "\"") + calib_blocks[b] + "\": " + buf;
+  }
+  return r + "}";
+}
+
+// the --perturb part of a run's JSON (empty without the flag)
+static std::string calib_nerr_json(const RunnerOptions &o, const RunSummary &s, const char *fmt) {
+  if (!o.perturb)
+    return "";
+  return ", \"perturb\": true, \"calib_nerr_first\": " + blocks_json(s.nerr_first, fmt) + ", \"calib_nerr_last\": " + blocks_json(s.nerr_last, fmt);
+}
 
 static std::string slam_json(const RunnerOptions &o, const RunSummary &s) {
   if (o.slam <= 0)
@@ -184,9 +234,10 @@ static const char *const backend_name = "oracle";
 static const char *const backend_name = "engine";
 #endif
 
-// one closed-loop run with measurement seed `seed_meas`; empty paths write nothing, capture_frame < 0 captures nothing,
-// consistency = record the consistency samples (written to consistency_path unless it is empty)
-static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<double, 8>> &traj_data, int seed_meas, const std::string &est_path,
+// one closed-loop run with measurement seed `seed_meas` and perturbation seed `seed_perturb`; empty paths write nothing,
+// capture_frame < 0 captures nothing, consistency = record the consistency samples (written to consistency_path unless it
+// is empty)
+static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<double, 8>> &traj_data, int seed_meas, int seed_perturb, const std::string &est_path,
                           const std::string &timing_path, bool consistency, const std::string &consistency_path, int capture_frame,
                           const std::string &capture_prefix, const std::string &slam_log_path = "") {
   SimParams sp;
@@ -194,8 +245,9 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
   sp.use_stereo = o.cams > 1;
   sp.num_pts = o.pts;
   sp.seed_state_init = o.seed_init;
-  sp.seed_preturb = o.seed_perturb;
+  sp.seed_preturb = seed_perturb;
   sp.seed_measurements = seed_meas;
+  sp.sim_do_perturbation = o.perturb;
   VioOptions vo;
   vo.num_cameras = o.cams;
   vo.max_clone_size = o.clones;
@@ -219,7 +271,7 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
   auto backend = std::make_shared<EngineCov>(cfg);
 #endif
 #endif
-  VioManager sys(vo, sp, backend);
+  VioManager sys(vo, sim.get_estimator_parameters(), backend);
   sys.record_slam_frames = !slam_log_path.empty();
   if (capture_frame >= 0) {
     // dump the marshalled inputs of ONE update (the golden "update case" wire format of tests/golden_io.py:
@@ -258,7 +310,7 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
       std::fclose(f);
     };
   }
-  SimRunResult res = run_simulation(sim, sys, o.frames, consistency);
+  SimRunResult res = run_simulation(sim, sys, o.frames, consistency || o.perturb);
   if (!est_path.empty()) {
     FILE *f = std::fopen(est_path.c_str(), "w");
     if (f) {
@@ -303,6 +355,10 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
     s.nees_ori += c.nees_ori, s.nees_pos += c.nees_pos;
   if (!res.consistency.empty())
     s.nees_ori /= (double)res.consistency.size(), s.nees_pos /= (double)res.consistency.size();
+  if (o.perturb && !res.consistency.empty()) {
+    calib_nerr(sys.state, res.consistency.front(), s.nerr_first);
+    calib_nerr(sys.state, res.consistency.back(), s.nerr_last);
+  }
   return s;
 }
 
@@ -318,7 +374,7 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
       const int seed = o.seed_meas + r;
       const std::string stem = out_dir.empty() ? std::string() : out_dir + "/";
       try {
-        out[(size_t)r] = run_one(o, traj_data, seed, stem.empty() ? "" : stem + "est_" + std::to_string(seed) + ".txt",
+        out[(size_t)r] = run_one(o, traj_data, seed, o.seed_perturb + r, stem.empty() ? "" : stem + "est_" + std::to_string(seed) + ".txt",
                                  stem.empty() || !timing ? "" : stem + "timing_" + std::to_string(seed) + ".csv", consistency,
                                  stem.empty() || !consistency ? "" : stem + "consistency_" + std::to_string(seed) + ".txt", -1, "");
       } catch (const std::exception &e) {
@@ -363,10 +419,14 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
       std::snprintf(buf, sizeof(buf), ", \"nees_ori\": %.17g, \"nees_pos\": %.17g", s.nees_ori, s.nees_pos);
       per_run += buf;
     }
-    per_run += slam_json(o, s) + "}";
+    if (o.perturb) {
+      std::snprintf(buf, sizeof(buf), ", \"seed_perturb\": %d", o.seed_perturb + r);
+      per_run += buf;
+    }
+    per_run += slam_json(o, s) + calib_nerr_json(o, s, "%.17g") + "}";
   }
   // the same statistics of the per-run mean NEES
-  std::string nees;
+  std::string stats;
   if (consistency) {
     double no = 0, np = 0, vno = 0, vnp = 0;
     for (const auto &s : out)
@@ -377,14 +437,33 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
     char buf[256];
     std::snprintf(buf, sizeof(buf), ", \"nees_ori_mean\": %.17g, \"nees_ori_std\": %.17g, \"nees_pos_mean\": %.17g, \"nees_pos_std\": %.17g", no,
                   std::sqrt(vno / runs), np, std::sqrt(vnp / runs));
-    nees = buf;
+    stats = buf;
+  }
+  // and of the per-block calibration errors
+  if (o.perturb) {
+    stats += ", \"perturb\": true";
+    for (int last = 0; last < 2; last++) {
+      double m[9] = {0}, sd[9] = {0};
+      for (const auto &s : out)
+        for (int b = 0; b < 9; b++)
+          m[b] += (last ? s.nerr_last : s.nerr_first)[b] / runs;
+      for (const auto &s : out)
+        for (int b = 0; b < 9; b++) {
+          const double d = (last ? s.nerr_last : s.nerr_first)[b] - m[b];
+          sd[b] += d * d / runs;
+        }
+      for (int b = 0; b < 9; b++)
+        sd[b] = std::sqrt(sd[b]);
+      const std::string key = last ? "calib_nerr_last" : "calib_nerr_first";
+      stats += ", \"" + key + "_mean\": " + blocks_json(m, "%.17g") + ", \"" + key + "_std\": " + blocks_json(sd, "%.17g");
+    }
   }
   std::printf("{\"backend\": \"%s\", \"runs\": %d, \"jobs\": %d, \"cams\": %d%s, \"max_clones\": %d, \"max_msckf_in_update\": %d, \"num_pts\": %d, \"calib\": %d, "
               "\"seed_init\": %d, \"seed_perturb\": %d, \"seed_meas\": %d, \"state_dim\": %d, \"map_points\": %zu, \"per_run\": [%s], "
               "\"ate_pos_m_mean\": %.17g, \"ate_pos_m_std\": %.17g, \"ate_ori_deg_mean\": %.17g, \"ate_ori_deg_std\": %.17g, \"frames_total\": %ld, "
               "\"wall_s\": %.6f, \"runs_per_s\": %.6f, \"frames_per_s\": %.3f%s}\n",
               backend_name, runs, jobs, o.cams, cam_model_json(o).c_str(), o.clones, o.msckf, o.pts, o.calib, o.seed_init, o.seed_perturb, o.seed_meas, out[0].state_dim, out[0].map_points,
-              per_run.c_str(), mp, std::sqrt(vp / runs), mo, std::sqrt(vo / runs), frames, wall, runs / wall, frames / wall, nees.c_str());
+              per_run.c_str(), mp, std::sqrt(vp / runs), mo, std::sqrt(vo / runs), frames, wall, runs / wall, frames / wall, stats.c_str());
   return 0;
 }
 
@@ -437,11 +516,16 @@ int main(int argc, char **argv) {
         o.feat_rep_slam = (int)(it - std::begin(rep_names));
     }
     else if (a == "--slam-log") slam_log_path = next();
+    else if (a == "--perturb") o.perturb = true;
   }
   if (!bad_slam.empty()) {
     std::fprintf(stderr, "malformed '%s': --slam takes an integer >= 0, --slam-in-update an integer >= 1, --slam-delay seconds >= 0, --feat-rep-slam one of "
                  "GLOBAL_3D GLOBAL_FULL_INVERSE_DEPTH ANCHORED_3D ANCHORED_FULL_INVERSE_DEPTH ANCHORED_MSCKF_INVERSE_DEPTH ANCHORED_INVERSE_DEPTH_SINGLE\n",
                  bad_slam.c_str());
+    return 2;
+  }
+  if (o.perturb && o.calib == 0) {
+    std::fprintf(stderr, "--perturb needs --calib 1: without online calibration the filter could not estimate the error it starts with\n");
     return 2;
   }
   if (runs > 0 && !slam_log_path.empty()) {
@@ -489,7 +573,7 @@ int main(int argc, char **argv) {
     return run_batch(o, traj_data, runs, jobs, out_dir, timing, consistency);
   }
   try {
-    const RunSummary s = run_one(o, traj_data, o.seed_meas, est_path, timing_path, consistency, consistency_path, capture_frame, capture_prefix, slam_log_path);
+    const RunSummary s = run_one(o, traj_data, o.seed_meas, o.seed_perturb, est_path, timing_path, consistency, consistency_path, capture_frame, capture_prefix, slam_log_path);
     char nees[128] = "";
     if (consistency)
       std::snprintf(nees, sizeof(nees), ", \"nees_ori\": %.12g, \"nees_pos\": %.12g", s.nees_ori, s.nees_pos);
@@ -498,7 +582,7 @@ int main(int argc, char **argv) {
                 "\"mean_ms_propagation\": %.4f, \"mean_ms_msckf_update\": %.4f, \"mean_ms_total\": %.4f, \"map_points\": %zu, \"status_hist\": [%ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld]%s}\n",
                 backend_name, s.frames, o.cams, cam_model_json(o).c_str(), o.clones, o.msckf, o.pts, o.calib, s.state_dim, s.ate_pos, s.ate_ori_deg, s.feats_in, s.feats_used, s.rows,
                 s.ms_prop, s.ms_msckf, s.ms_total, s.map_points, s.status_hist[0], s.status_hist[1], s.status_hist[2], s.status_hist[3], s.status_hist[4],
-                s.status_hist[5], s.status_hist[6], s.status_hist[7], s.status_hist[8], (nees + slam_json(o, s)).c_str());
+                s.status_hist[5], s.status_hist[6], s.status_hist[7], s.status_hist[8], (nees + slam_json(o, s) + calib_nerr_json(o, s, "%.12g")).c_str());
   } catch (const std::exception &e) {
     std::fprintf(stderr, "run_simulation failed: %s\n", e.what());
     return 1;
