@@ -1,4 +1,4 @@
-// chol_tiles.cuh — in-CTA Cholesky of a tile-packed lower triangle on the FP64 tensor-core path (DMMA m8n8k4).
+// chol_tiles.cuh — in-CTA Cholesky of a tile-packed lower triangle on the FP64 tensor-core path (DMMA, mma.sync .f64).
 // Shared by the CholeskyQR2 / EKF factor kernels (k_cholqr.cu) and the per-feature chi² gate (k_feature.cu).
 //
 // Layout: the lower triangle is cut into 8x8 tiles; tile (bi, bj), bj <= bi, lives at (bi(bi+1)/2 + bj)*64 doubles, row-major.
@@ -18,6 +18,22 @@
 // D(8x8) += A(8x4) B(4x8). a = A[lane>>2][lane&3], b = B[lane&3][lane>>2], d0/d1 = D[lane>>2][2*(lane&3)+{0,1}]
 __device__ __forceinline__ void ct_dmma(double &d0, double &d1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
+}
+// Two m8n8k4 products that share B in one instruction: [D0; D1](16x8) += [A0; A1](16x4) B(4x8), m16n8k4. Same operand and
+// accumulator fragments as ct_dmma (a0/d0/d1 of A0/D0, a1/e0/e1 of A1). It takes the FP64 pipe as long as one m8n8k4 does
+// (twice the rate, tools/ubench/fp64_rate.cu) and gives the same bits as the two m8n8k4 it replaces.
+__device__ __forceinline__ void ct_dmma2(double &d0, double &d1, double &e0, double &e1, double a0, double a1, double b) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+               : "+d"(d0), "+d"(d1), "+d"(e0), "+d"(e1)
+               : "d"(a0), "d"(a1), "d"(b));
+}
+// Two 8x8x8 tile products that share B, m16n8k8: [D0; D1] += [A0; A1] B with k = 0..7. The operands are two ct_dmma
+// k-steps each: a00/a01 = A0's fragments at k 0-3 / 4-7, likewise a10/a11 of A1 and b0/b1 of B. Same bits as the chain
+// ct_dmma(k 0-3), ct_dmma(k 4-7) on each tile, in half the pipe time.
+__device__ __forceinline__ void ct_dmma2k8(double &d0, double &d1, double &e0, double &e1, double a00, double a01, double a10, double a11, double b0, double b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+d"(d0), "+d"(d1), "+d"(e0), "+d"(e1)
+               : "d"(a00), "d"(a10), "d"(a01), "d"(a11), "d"(b0), "d"(b1));
 }
 __device__ __forceinline__ int ct_tri(int b) { return (b * (b + 1)) >> 1; }
 __device__ __forceinline__ void ct_bar_group(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
@@ -144,18 +160,24 @@ __device__ __forceinline__ void ct_linv8(const double *Lt, const double *invd, d
   }
 }
 
-// Panel tile (i, k): X = T(i,k) L_kk^-T as one 8x8x8 product on the tensor path, written back over the tile and into the
-// operand buffer (rows 8i.. of Xb). The whole warp calls.
-__device__ __forceinline__ void ct_panel_tile(const CtView &sm, int i, int k, const double *Linv, double *Xb) {
+// Panel tiles (i, k) and (i1, k): X = T(i,k) L_kk^-T, each one 8x8x8 product on the tensor path (both in one m16n8k8:
+// they share L_kk^-T), written back over the tile and into the operand buffer (rows 8i.. of Xb). two == false: tile i1
+// does not exist; its half of the product runs on zero operands and is dropped. The whole warp calls.
+__device__ __forceinline__ void ct_panel_pair(const CtView &sm, int i, int i1, bool two, int k, const double *Linv, double *Xb) {
   const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
   double *t = sm.T + (size_t)(ct_tri(i) + k) * 64;
+  double *t1 = sm.T + (size_t)(ct_tri(i1) + k) * 64;
   const double a0 = t[g * 8 + q], a1 = t[g * 8 + q + 4];
+  const double a10 = two ? t1[g * 8 + q] : 0.0, a11 = two ? t1[g * 8 + q + 4] : 0.0;
   const double b0 = Linv[g * 8 + q], b1 = Linv[g * 8 + q + 4]; // B[k][n] = Linv[n][k]
-  double2 d = make_double2(0.0, 0.0);
-  ct_dmma(d.x, d.y, a0, b0);
-  ct_dmma(d.x, d.y, a1, b1);
+  double2 d = make_double2(0.0, 0.0), e = make_double2(0.0, 0.0);
+  ct_dmma2k8(d.x, d.y, e.x, e.y, a0, a1, a10, a11, b0, b1);
   *reinterpret_cast<double2 *>(t + 2 * lane) = d;
   *reinterpret_cast<double2 *>(Xb + (size_t)(8 * i + g) * CT_XP + 2 * q) = d;
+  if (two) {
+    *reinterpret_cast<double2 *>(t1 + 2 * lane) = e;
+    *reinterpret_cast<double2 *>(Xb + (size_t)(8 * i1 + g) * CT_XP + 2 * q) = e;
+  }
 }
 
 // rows i0, i0+stride, ... of panel k: x L_kk' = S[i][kb..kb+8) by substitution, one thread per row (backward stable row by
@@ -235,9 +257,11 @@ __device__ __forceinline__ void ct_tile_mma(CtTileOps &o) {
   ct_dmma(o.c.x, o.c.y, o.a0, o.b0);
   ct_dmma(o.c.x, o.c.y, o.a1, o.b1);
 }
-__device__ __forceinline__ void ct_tile_mma_store(CtTileOps &o) {
-  ct_tile_mma(o);
-  *o.cp = o.c;
+// two tiles of one block column (same B operands) in one m16n8k8
+__device__ __forceinline__ void ct_tile_pair_mma_store(CtTileOps &o0, CtTileOps &o1) {
+  ct_dmma2k8(o0.c.x, o0.c.y, o1.c.x, o1.c.y, o0.a0, o0.a1, o1.a0, o1.a1, o0.b0, o0.b1);
+  *o0.cp = o0.c;
+  *o1.cp = o1.c;
 }
 
 #ifdef CQ_PROBE
@@ -247,7 +271,8 @@ __device__ __forceinline__ void ct_tile_mma_store(CtTileOps &o) {
 #endif
 
 // One row of the trailing update of step k: T(bi, bj) -= X(bi,k) X(bj,k)' for j0 <= bj <= jmax. The row's own operand
-// fragments stay in registers; two tiles in flight.
+// fragments stay in registers; two tiles in flight. The tiles of a row share A, not B, so they stay m8n8k4: pairing the
+// two rows of a warp by block column (m16n8k8) made k_cq_chol_gram slower (74.7 -> 77.1 us per two launches, config 2).
 __device__ __forceinline__ void ct_trail_row(const CtView &sm, const double *Xk, int bi, int j0, int jmax, int lane) {
   const int g = lane >> 2, q = lane & 3;
   const double *xa = Xk + (size_t)(8 * bi + g) * CT_XP + q;
@@ -353,8 +378,8 @@ __device__ __forceinline__ void ct_chol_tiles(const CtView &sm, int n, int nrows
     } else if (helper) {
       if (LINV) {
         const double *Lk = par ? sm.Linv1 : sm.Linv0;
-        for (int i = k + 2 + hr; i < NRB; i += NH)
-          ct_panel_tile(sm, i, k, Lk, Xk);
+        for (int i = k + 2 + hr; i < NRB; i += 2 * NH)
+          ct_panel_pair(sm, i, i + NH, i + NH < NRB, k, Lk, Xk);
       } else {
         ct_panel_rows(sm.T, Xk, sm.invd, 8 * (k + 2) + hr * 32 + lane, NH * 32, nrows, k, min(8, n - 8 * k));
       }
@@ -368,8 +393,7 @@ __device__ __forceinline__ void ct_chol_tiles(const CtView &sm, int n, int nrows
           CtTileOps o0, o1;
           ct_tile_load(o0, sm, Xk, i, k + 1, lane, true);
           ct_tile_load(o1, sm, Xk, i + NH, k + 1, lane, i + NH < NRB);
-          ct_tile_mma_store(o0);
-          ct_tile_mma_store(o1);
+          ct_tile_pair_mma_store(o0, o1);
         }
         asm volatile("bar.arrive 2, %0;" ::"r"((NH + 1) * 32) : "memory");
         CT_PROBE_T(p2);

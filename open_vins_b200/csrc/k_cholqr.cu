@@ -158,11 +158,12 @@ __device__ __forceinline__ void cq_gram_kstep(double (&acc)[4][4][2], const doub
     for (int b = 0; b < 4; b++)
       fb[b] = row[offJ + 8 * b];
   }
+  // output blocks a and a+1 share fb[b]: one m16n8k4 each pair
 #pragma unroll
-  for (int a = 0; a < 4; a++)
+  for (int a = 0; a < 4; a += 2)
 #pragma unroll
     for (int b = 0; b < 4; b++)
-      dmma(acc[a][b][0], acc[a][b][1], fa[a], fb[b]);
+      ct_dmma2(acc[a][b][0], acc[a][b][1], acc[a + 1][b][0], acc[a + 1][b][1], fa[a], fa[a + 1], fb[b]);
 }
 
 } // namespace
@@ -1162,10 +1163,10 @@ __global__ void __launch_bounds__(CQ_GN_T) k_cq_gemm_nt(double *__restrict__ C, 
       for (int b = 0; b < 2; b++)
         fb[b] = Bs[wn + 8 * b + g][4 * ks + q];
 #pragma unroll
-      for (int a = 0; a < 4; a++)
+      for (int a = 0; a < 4; a += 2)
 #pragma unroll
         for (int b = 0; b < 2; b++)
-          dmma(acc[a][b][0], acc[a][b][1], fa[a], fb[b]);
+          ct_dmma2(acc[a][b][0], acc[a][b][1], acc[a + 1][b][0], acc[a + 1][b][1], fa[a], fa[a + 1], fb[b]);
     }
     __syncthreads();
   }

@@ -11,7 +11,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, "open_vins_b200", "libovb200.so")
 out = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
-WATCH = ["DMMA", "DFMA", "DMUL", "DADD", "MUFU.RSQ64H", "MUFU.RCP64H", "LDGSTS", "UBLKCP", "SYNCS", "SHFL", "BAR", "LDS", "STS", "UTMALDG", "HGMMA", "IGMMA", "QGMMA"]
+WATCH = ["DMMA.8x8x4", "DMMA.16x8x4", "DMMA.16x8x8", "DMMA.16x8x16", "DFMA", "DMUL", "DADD", "MUFU.RSQ64H", "MUFU.RCP64H", "LDGSTS", "UBLKCP", "SYNCS", "SHFL", "BAR", "LDS", "STS", "UTMALDG", "HGMMA", "IGMMA", "QGMMA"]
 counts = collections.OrderedDict()
 fn = None
 for line in out.splitlines():
@@ -20,7 +20,7 @@ for line in out.splitlines():
         fn = m.group(1)
         counts[fn] = collections.Counter()
         continue
-    m = re.match(r"\s+/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
+    m = re.match(r"\s+/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Za-z0-9_.]+)", line)
     if m and fn:
         op = m.group(1)
         for w in WATCH:
@@ -30,7 +30,7 @@ for line in out.splitlines():
 demangle = subprocess.run(["c++filt"], input="\n".join(counts.keys()), capture_output=True, text=True).stdout.splitlines()
 with open(os.path.join(ROOT, "profiles", "sass.txt"), "w") as f:
     f.write("# SASS opcode counts per kernel of open_vins_b200/libovb200.so (cuobjdump -sass, sm_90a); regenerate: python tools/sass_listing.py\n")
-    f.write("# DMMA = mma.sync.m8n8k4.f64 (FP64 tensor-core path); LDGSTS = cp.async; MUFU.RSQ64H = rsqrt.approx.f64 pivot seed.\n")
+    f.write("# DMMA.8x8x4 / .16x8x4 / .16x8x8 / .16x8x16 = mma.sync.m8n8k4 / m16n8k4 / m16n8k8 / m16n8k16 .f64 (FP64 tensor-core path); LDGSTS = cp.async; MUFU.RSQ64H = rsqrt.approx.f64 pivot seed.\n")
     f.write("# UBLKCP = cp.async.bulk (TMA engine, 1-D) + SYNCS = mbarrier ops: the packed Cholesky factor of k_cq_trsm. wgmma / tensor-map TMA opcodes\n# (HGMMA, IGMMA, QGMMA, UTMALDG): none — wgmma has no FP64 kind, and every other operand tile here is\n")
     f.write("# either register-resident or a few KB staged by cp.async (DESIGN.md §4).\n")
     for (fn, c), dm in zip(counts.items(), demangle):
