@@ -491,8 +491,12 @@ ovb_status ovb_cov_propagate(ovb_ctx *ctx, int new_off, int p, const int *old_of
       return OVB_ERR_ARG;
     q += old_sz[i];
   }
-  if (q > ctx->cfg.max_state || p > ctx->cfg.max_state || (size_t)p * q + (size_t)p * p > ctx->Hs_cap)
+  // d_Hs holds [Phi p*q][Q p*p] doubles, then the q int32 old indices (ceil(q/2) doubles)
+  if (q > ctx->cfg.max_state || p > ctx->cfg.max_state || (size_t)p * q + (size_t)p * p + ((size_t)q + 1) / 2 > ctx->Hs_cap) {
+    snprintf(ctx->err, sizeof(ctx->err), "ovb_cov_propagate: p=%d, q=%d exceed the staging matrix (max_state=%d, %zu doubles)", p, q,
+             ctx->cfg.max_state, ctx->Hs_cap);
     return OVB_ERR_CAPACITY;
+  }
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
   // stage: [Phi p*q][Q p*p] doubles, then q ints
   {
