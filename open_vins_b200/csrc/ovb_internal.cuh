@@ -214,7 +214,7 @@ struct ovb_ctx {
   int max_rows;
   int sm_count;
   size_t info_bytes; // DevUpdateInfo rounded up: d_dx / h_dx start right behind d_info / h_info
-  int attr_done[8]; // per-context (= per-device) one-time cudaFuncSetAttribute flags: 0 tsqr, 1 feature, 2 ekf, 3 gram, 4 cholqr
+  int attr_done[9]; // per-context (= per-device) one-time cudaFuncSetAttribute flags: 0 tsqr, 1 feature, 2 ekf, 3 gram, 4 cholqr, 8 triangulate
   int tsqr_pdl;     // programmatic dependent launch between the TSQR level kernels (OVB_TSQR_PDL=0 disables: A/B timing only)
   int tsqr_cluster; // upper TSQR levels as one thread-block cluster (OVB_TSQR_CLUSTER=0 disables: A/B timing only)
   int gram_cluster;  // k_cq_gram: clusters of 4 slabs pre-reduce in distributed shared memory (OVB_GRAM_CLUSTER=0 disables: A/B timing only)
