@@ -446,7 +446,8 @@ ovb_status ovb_msckf_shard_finish(ovb_ctx *ctx, double *stacked_dev, int n_block
  * re-enqueues the identical device pipeline `steps` times (optionally flushing L2 with a 256 MiB memset between steps),
  * timing each step with CUDA events on the context stream. ms_per_step[steps]; stage_ms_sum[5] = summed stage times
  * {triangulate, feature systems, column map, compression, EKF update}. This is bench.py's kernel-only `value` leg. */
-/* out[0] kernels launched by the last update pipeline, out[1] of which TSQR level kernels,
+/* out[0] kernels launched by the last call that launches any (ovb_msckf_shard_finish adds to its
+ * ovb_msckf_shard_compress), counted at the launch, out[1] of which TSQR level kernels,
  * out[2]/out[3] bytes copied host->device / device->host by the last ovb_msckf_update. */
 ovb_status ovb_last_counters(const ovb_ctx *ctx, int64_t out[4]);
 /* The last ovb_slam_delayed_init[_reps] call: out[0] features that reached StateHelper::initialize (triangulated), out[1]
@@ -456,9 +457,10 @@ ovb_status ovb_last_init_counters(const ovb_ctx *ctx, int64_t out[4]);
 /* Host wall clock (microseconds) of the last ovb_msckf_update: [0] marshalling into the pinned arena + H2D enqueue,
  * [1] kernel and D2H enqueue, [2] wait for the stream, [3] unpacking the results. */
 ovb_status ovb_last_host_us(const ovb_ctx *ctx, double out[4]);
-/* Per-kernel timing (measurement support): ovb_set_profile(ctx,1) brackets every kernel of the update pipeline that is
- * launched on the context stream with CUDA events (programmatic dependent launch is off meanwhile); ovb_profile_read
- * returns the kernels of the last update in launch order: NUL-separated mangled names and durations in microseconds. */
+/* Per-kernel timing (measurement support): ovb_set_profile(ctx,1) brackets every kernel launch with CUDA events
+ * (programmatic dependent launch is off meanwhile); ovb_profile_read returns the kernels of the last call (as counted by
+ * ovb_last_counters) in launch order: NUL-separated mangled names and durations in microseconds, the first cap of them;
+ * *n = the number of kernels of that call, which may exceed cap. */
 ovb_status ovb_set_profile(ovb_ctx *ctx, int enabled);
 ovb_status ovb_profile_read(ovb_ctx *ctx, char *names, int name_cap, float *us, int cap, int *n);
 ovb_status ovb_set_replay(ovb_ctx *ctx, int enabled);

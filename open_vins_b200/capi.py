@@ -646,11 +646,16 @@ class Engine:
         self._check(self.lib.ovb_set_profile(self.h, int(bool(enabled))))
 
     def profile_read(self):
-        """[(kernel name, microseconds)] of the last update, in launch order (main-stream kernels)."""
-        buf = C.create_string_buffer(16384)
-        us = np.zeros(96, dtype=np.float32)
-        n = np.zeros(1, dtype=np.int32)
-        self._check(self.lib.ovb_profile_read(self.h, buf, len(buf), _ptr(us, c_float_p), 96, _ptr(n, c_int_p)))
+        """[(kernel name, microseconds)] of every kernel the last call launched, in launch order."""
+        cap = 128
+        while True:
+            buf = C.create_string_buffer(512 * cap)  # mangled names of templated kernels run to a few hundred bytes
+            us = np.zeros(cap, dtype=np.float32)
+            n = np.zeros(1, dtype=np.int32)
+            self._check(self.lib.ovb_profile_read(self.h, buf, len(buf), _ptr(us, c_float_p), cap, _ptr(n, c_int_p)))
+            if int(n[0]) <= cap:
+                break
+            cap = int(n[0])
         names = buf.raw.split(b"\0")[: int(n[0])]
         return [(nm.decode(), float(us[i])) for i, nm in enumerate(names)]
 

@@ -295,6 +295,7 @@ OVB_HD bool anchor_change(const AnchorFrame &fr, bool do_fej, bool ext, int rep,
 // kernels after this one then return without reading Phi, the indices or P.
 __global__ void k_anchor_phi(const DevWinFrame *__restrict__ wf, const DevWinLM *__restrict__ lms, int n, int do_fej, int ext, int *flags,
                              double *__restrict__ new_values, double *__restrict__ phi, int *__restrict__ idx, int *__restrict__ q_out) {
+  OVB_PDL_ENTER();
   const int l = blockIdx.x * blockDim.x + threadIdx.x;
   if (l >= n)
     return;
@@ -322,7 +323,7 @@ __global__ void k_anchor_phi(const DevWinFrame *__restrict__ wf, const DevWinLM 
 
 void launch_anchor_phi(ovb_ctx *ctx, const DevWinFrame *wf, const DevWinLM *lms, int n, int do_fej, int ext, int *flags, double *new_values,
                        double *phi, int *idx, int *q) {
-  k_anchor_phi<<<(n + 63) / 64, 64, 0, ctx->stream>>>(wf, lms, n, do_fej, ext, flags, new_values, phi, idx, q);
+  ovb_launch(ctx, k_anchor_phi, dim3((n + 63) / 64), dim3(64), (size_t)0, wf, lms, n, do_fej, ext, flags, new_values, phi, idx, q);
 }
 
 extern "C" ovb_status ovb_slam_anchor_change(const ovb_frame *fr, const ovb_opts *op, int lm_off, const double *value, const double *value_fej,

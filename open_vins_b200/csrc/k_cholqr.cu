@@ -1256,39 +1256,6 @@ __global__ void __launch_bounds__(256) k_cq_trmm_wide(const double *__restrict__
 
 // ------------------------------------------------------------------------------------------------------------ launchers
 #define CQ_GRAM_CS 4 // slabs per cluster in k_cq_gram
-// launch k_cq_gram over nslab_padded slabs (a multiple of CQ_GRAM_CS) as clusters of CQ_GRAM_CS along y
-static void cq_launch_gram(ovb_ctx *ctx, int nblk, int nslab_padded, size_t smem, const double *A, int ldA, int m, int nt, int slab_rows, int BW, int nblk_side,
-                           double *Gpart, int cs) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(nblk, nslab_padded);
-  cfg.blockDim = dim3(CQ_GRAM_T);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = ctx->stream;
-  cudaLaunchAttribute at[2];
-  int na = 0;
-  if (ctx->tsqr_pdl && !ctx->prof_on) {
-    at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[na].val.programmaticStreamSerializationAllowed = 1;
-    na++;
-  }
-  if (cs > 1) {
-    at[na].id = cudaLaunchAttributeClusterDimension;
-    at[na].val.clusterDim.x = 1;
-    at[na].val.clusterDim.y = cs;
-    at[na].val.clusterDim.z = 1;
-    na++;
-  }
-  cfg.attrs = at;
-  cfg.numAttrs = na;
-  const bool prof = ctx->prof_on && ctx->prof_n < 96 && ctx->prof_ev[0] != nullptr;
-  if (prof)
-    cudaEventRecord(ctx->prof_ev[2 * ctx->prof_n], ctx->stream);
-  cudaLaunchKernelEx(&cfg, k_cq_gram, A, ldA, m, nt, slab_rows, BW, nblk_side, Gpart, cs);
-  if (prof) {
-    cudaEventRecord(ctx->prof_ev[2 * ctx->prof_n + 1], ctx->stream);
-    ctx->prof_fn[ctx->prof_n++] = (const void *)k_cq_gram;
-  }
-}
 
 static bool cq_attrs(ovb_ctx *ctx) {
   if (!ctx->attr_done[4]) {
@@ -1461,10 +1428,10 @@ bool launch_chol_solve_wide(ovb_ctx *ctx, double *S, int ldS, int r, double *w, 
 }
 
 // wide CholeskyQR2: same scheme as below with the blocked factorisation / solve
-static int cq_compress_wide(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR) {
+static bool cq_compress_wide(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR) {
   const int nt = n + 1;
   if (nt > CQ_WMAX - 7 || !cq_ensure_wide(ctx))
-    return -1;
+    return false;
   const int nT = (nt + 31) / 32, BW = 4, nblk_side = (nT + BW - 1) / BW, nblk = nblk_side * (nblk_side + 1) / 2;
   int nslab = ctx->sm_count / nblk;
   if (nslab < 1)
@@ -1480,37 +1447,34 @@ static int cq_compress_wide(ovb_ctx *ctx, double *A, int m, int n, int ldA, doub
       cudaFree(ctx->d_Gpart);
     ctx->d_Gpart = nullptr;
     if (cudaMalloc(&ctx->d_Gpart, sizeof(double) * need_part) != cudaSuccess)
-      return -1;
+      return false;
     ctx->Gpart_cap = need_part;
   }
   double *G1 = ctx->d_cqw, *G2 = G1 + (size_t)CQ_WMAX * CQ_WMAX, *Lpk1 = G2 + (size_t)CQ_WMAX * CQ_WMAX, *Lpk2 = Lpk1 + (size_t)CQ_WBLOCKS * CQ_PK_DOUBLES;
   double *floor_dev = Lpk2 + (size_t)CQ_WBLOCKS * CQ_PK_DOUBLES;
   const size_t gram_smem = sizeof(double) * 2 * CQ_KB * (size_t)(2 * BW * 32 + 4);
-  int launches = 0;
   for (int pass = 0; pass < 2; pass++) {
     double *G = pass == 0 ? G1 : G2;
-    cq_launch_gram(ctx, nblk, nslab, gram_smem, (const double *)A, ldA, m, nt, slab_rows, BW, nblk_side, ctx->d_Gpart, 1);
+    ovb_launch(ctx, k_cq_gram, dim3(nblk, nslab), dim3(CQ_GRAM_T), gram_smem, A, ldA, m, nt, slab_rows, BW, nblk_side, ctx->d_Gpart, 1);
     ovb_launch(ctx, k_cq_reduce, dim3(CQ_RED_GX, nblk), dim3(CQ_RED_T), (size_t)0, (const double *)ctx->d_Gpart, nslab, nblk, BW, nblk_side, nt, G, (int)CQ_WMAX, 0);
     ovb_launch(ctx, k_cq_shift, dim3(1), dim3(256), (size_t)0, G, (int)CQ_WMAX, nt, pass == 0 ? 1e-11 : 1e-13, floor_dev + pass);
     cq_chol_blocked(ctx, G, CQ_WMAX, nt, 0, pass == 0 ? Lpk1 : Lpk2, floor_dev + pass, (DevUpdateInfo *)nullptr);
     if (pass == 0)
       cq_trsm_blocked(ctx, A, ldA, m, nt, G1, CQ_WMAX, Lpk1);
-    launches += 3 + 3 * ((nt + CQ_WB - 1) / CQ_WB);
   }
   const int nT32 = (nt + 31) / 32;
   ovb_launch(ctx, k_cq_trmm_wide, dim3(nT32, nT32), dim3(256), (size_t)0, (const double *)G2, (const double *)G1, (int)CQ_WMAX, nt, Rout, ldR);
-  ctx->n_launch += launches + 1;
-  return launches + 1;
+  return true;
 }
 
 // [R | z] <- shifted CholeskyQR2 of A [m x (n+1)]: pass 1 k_cq_gram -> k_cq_reduce -> k_cq_chol_gram, pass 2
 // k_cq_solve_gram (Q1 = A R1^-1 and its Gram partials in one kernel) -> k_cq_reduce -> k_cq_chol_gram, then k_cq_trmm.
-// A is left unchanged here (the wide path overwrites it with Q1). Returns the number of kernels launched, or -1 when the
-// system is too wide for this path (the caller falls back to the Householder TSQR).
-int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR) {
+// A is left unchanged here (the wide path overwrites it with Q1). Returns false when the system is too wide for this
+// path (the caller falls back to the Householder TSQR).
+bool launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR) {
   const int nt = n + 1;
   if ((ldA & 1) || m < 1)
-    return -1;
+    return false;
   cq_attrs(ctx);
   if (nt > CQ_MAXN)
     return cq_compress_wide(ctx, A, m, n, ldA, Rout, ldR);
@@ -1530,7 +1494,7 @@ int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, doub
   const size_t need_part = part_doubles + cq_solve_gram_scratch(nslab, nt, BW, slab_rows); // partials | pass-2 row scratch
   const int ldW = CQ_MAXN + 8;
   if (!cq_ensure_G(ctx))
-    return -1;
+    return false;
   if (need_part > ctx->Gpart_cap) {
     // the stacked rows grow over a run's first ~30 updates; taking half as much again keeps regrowth to a few early
     // updates (cudaFree waits for the whole device, other contexts' work included: tools/monte_carlo_timing.py)
@@ -1540,7 +1504,7 @@ int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, doub
     ctx->d_Gpart = nullptr;
     ctx->Gpart_cap = 0;
     if (cudaMalloc(&ctx->d_Gpart, sizeof(double) * cap) != cudaSuccess)
-      return -1;
+      return false;
     ctx->Gpart_cap = cap;
   }
   double *G = ctx->d_G, *L1 = G + (size_t)ldW * ldW, *L2 = L1 + (size_t)ldW * ldW;
@@ -1549,7 +1513,8 @@ int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, doub
   if (cs > 1 && gram_smem < sizeof(double) * 16 * 1024)
     gram_smem = sizeof(double) * 16 * 1024; // staging of the 16 warp tiles for the cluster reduction
   // pass 1: G1 = A'A -> R1
-  cq_launch_gram(ctx, nblk, nslab_pad, gram_smem, (const double *)A, ldA, m, nt, slab_rows, BW, nblk_side, ctx->d_Gpart, cs);
+  ovb_launch(ctx, k_cq_gram, ovb_grid(dim3(nblk, nslab_pad), dim3(1, cs, 1)), dim3(CQ_GRAM_T), gram_smem, A, ldA, m, nt, slab_rows, BW, nblk_side,
+             ctx->d_Gpart, cs);
   ovb_launch(ctx, k_cq_reduce, dim3(CQ_RED_GX, nblk), dim3(CQ_RED_T), (size_t)0, (const double *)ctx->d_Gpart, npart, nblk, BW, nblk_side, nt, G, ldW, 1);
   const unsigned long long epoch = ++ctx->pub_epoch; // R1 streams into k_cq_solve_gram
   ovb_launch(ctx, k_cq_chol_gram, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), (const double *)G, ldW, nt, 1e-11, L1, 1, ctx->d_pub, epoch);
@@ -1559,6 +1524,5 @@ int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, doub
   ovb_launch(ctx, k_cq_chol_gram, dim3(1), dim3(CQ_CHOL_T), sizeof(CqCholSmem), (const double *)G, ldW, nt, 1e-13, L2, 1, (unsigned long long *)nullptr, 0ull);
   const int nT16 = (nt + 15) / 16;
   ovb_launch(ctx, k_cq_trmm, dim3(nT16, nT16), dim3(256), (size_t)0, (const double *)L2, (const double *)L1, nt, Rout, ldR);
-  ctx->n_launch += 7;
-  return 7;
+  return true;
 }

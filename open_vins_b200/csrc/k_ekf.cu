@@ -493,6 +493,7 @@ __global__ void k_cov_init_augment(double *__restrict__ P, int ld, int N, int k,
                                    const double *__restrict__ Hx, const double *__restrict__ Hinv, double sigma2, const int *__restrict__ skip) {
   extern __shared__ double ism[]; // m[N][k], then M[k][k]
   double *m = ism, *M = ism + (size_t)N * k;
+  OVB_PDL_ENTER();
   const int tid = threadIdx.x;
   if (skip && *skip)
     return;
@@ -552,14 +553,15 @@ bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, c
     cudaFuncSetAttribute(k_cov_init_augment, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     ctx->attr_done[5] = 1;
   }
-  k_cov_init_augment<<<1, 256, smem, ctx->stream>>>(ctx->P[ctx->cur], ctx->ldP, N, k, n, ctx->d_info, Hx_dev, Hinv_dev, sigma2, skip_dev);
-  return cudaGetLastError() == cudaSuccess;
+  return ovb_launch(ctx, k_cov_init_augment, dim3(1), dim3(256), smem, ctx->P[ctx->cur], ctx->ldP, N, k, n, ctx->d_info, Hx_dev, Hinv_dev, sigma2,
+                    skip_dev) == cudaSuccess;
 }
 
 // ovb_slam_delayed_init, after the per-feature kernel: the head of the init system (status, chi2, skip flag), H_L^-1 of the
 // k x k invertible block by Gauss-Jordan with partial pivoting (the host's order in ovb_cov_initialize), dx_new = H_L^-1 r,
 // and the column map for the augmentation and the EKF update. H_L is rows/columns 3-k..2 of the kernel's 3 x 3 block.
 __global__ void k_init_prep(const DevFeat *__restrict__ feat, DevInitSys *__restrict__ sys, DevUpdateInfo *__restrict__ info, int k, int n) {
+  OVB_PDL_ENTER();
   const int tid = threadIdx.x;
   const bool ok = feat->status == OVB_FEAT_OK;
   if (ok)
@@ -624,12 +626,13 @@ __global__ void k_init_prep(const DevFeat *__restrict__ feat, DevInitSys *__rest
 }
 
 void launch_init_prep(ovb_ctx *ctx, int feat, int k, int n) {
-  k_init_prep<<<1, 256, 0, ctx->stream>>>(ctx->d_feat + feat, ctx->d_init, ctx->d_info, k, n);
+  ovb_launch(ctx, k_init_prep, dim3(1), dim3(256), (size_t)0, ctx->d_feat + feat, ctx->d_init, ctx->d_info, k, n);
 }
 
 // StateHelper::clone: append a copy of the `size`-wide variable at old_off (StateHelper.cpp:371-373)
 // neg_diag (optional): the flag of a propagation enqueued before; a negative diagonal there cancels the clone
 __global__ void k_cov_clone(double *P, int ld, int N, int old_off, int size, const int *neg_diag) {
+  OVB_PDL_ENTER();
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   int N2 = N + size;
   if (idx >= N2 * size || (neg_diag && *neg_diag != OVB_NO_NEG_DIAG))
@@ -647,6 +650,7 @@ __global__ void k_cov_clone(double *P, int ld, int N, int old_off, int size, con
 }
 // augment_clone time-offset term, step 1: P[:, N..N+size) += P[:, dt] dnc'   (StateHelper.cpp:611-612)
 __global__ void k_cov_dt_cols(double *P, int ld, int N2, int new_off, int size, int dt_off, const double *dnc, const int *neg_diag) {
+  OVB_PDL_ENTER();
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= N2 * size || (neg_diag && *neg_diag != OVB_NO_NEG_DIAG))
     return;
@@ -655,6 +659,7 @@ __global__ void k_cov_dt_cols(double *P, int ld, int N2, int new_off, int size, 
 }
 // step 2: P[N..N+size, :] += dnc P[dt, :]   (StateHelper.cpp:613-614) — reads the row written by step 1
 __global__ void k_cov_dt_rows(double *P, int ld, int N2, int new_off, int size, int dt_off, const double *dnc, const int *neg_diag) {
+  OVB_PDL_ENTER();
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= N2 * size || (neg_diag && *neg_diag != OVB_NO_NEG_DIAG))
     return;
@@ -666,16 +671,18 @@ void launch_cov_clone(ovb_ctx *ctx, int old_off, int size, const double *dnc_dt_
   double *P = ctx->P[ctx->cur];
   int N = ctx->N, N2 = N + size;
   int tot = N2 * size;
-  k_cov_clone<<<(tot + 255) / 256, 256, 0, ctx->stream>>>(P, ctx->ldP, N, old_off, size, neg_diag_dev);
+  const dim3 grid((tot + 255) / 256), block(256);
+  ovb_launch(ctx, k_cov_clone, grid, block, (size_t)0, P, ctx->ldP, N, old_off, size, neg_diag_dev);
   if (dnc_dt_dev) {
-    k_cov_dt_cols<<<(tot + 255) / 256, 256, 0, ctx->stream>>>(P, ctx->ldP, N2, N, size, dt_off, dnc_dt_dev, neg_diag_dev);
-    k_cov_dt_rows<<<(tot + 255) / 256, 256, 0, ctx->stream>>>(P, ctx->ldP, N2, N, size, dt_off, dnc_dt_dev, neg_diag_dev);
+    ovb_launch(ctx, k_cov_dt_cols, grid, block, (size_t)0, P, ctx->ldP, N2, N, size, dt_off, dnc_dt_dev, neg_diag_dev);
+    ovb_launch(ctx, k_cov_dt_rows, grid, block, (size_t)0, P, ctx->ldP, N2, N, size, dt_off, dnc_dt_dev, neg_diag_dev);
   }
 }
 
 // StateHelper::marginalize (StateHelper.cpp:293-313): out of place into the other buffer; the x2-x1 block is the
 // transpose of the copied x1-x2 block exactly as the reference builds it.
 __global__ void k_cov_marg(const double *Pin, double *Pout, int ld, int N, int off, int size) {
+  OVB_PDL_ENTER();
   int N2 = N - size;
   int i = blockIdx.y * blockDim.y + threadIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N2 || j >= N2)
@@ -688,7 +695,7 @@ __global__ void k_cov_marg(const double *Pin, double *Pout, int ld, int N, int o
 void launch_cov_marginalize(ovb_ctx *ctx, int off, int size) {
   int N2 = ctx->N - size;
   dim3 b(32, 8), g((N2 + 31) / 32, (N2 + 7) / 8);
-  k_cov_marg<<<g, b, 0, ctx->stream>>>(ctx->P[ctx->cur], ctx->P[ctx->cur ^ 1], ctx->ldP, ctx->N, off, size);
+  ovb_launch(ctx, k_cov_marg, g, b, (size_t)0, ctx->P[ctx->cur], ctx->P[ctx->cur ^ 1], ctx->ldP, ctx->N, off, size);
 }
 
 // EKFPropagation (StateHelper.cpp:80-100). old_idx[k] = covariance index of Phi's column k (q of them).
@@ -709,6 +716,7 @@ __device__ __forceinline__ double prop_PCP_entry(double acc, int i, int j, int q
   return acc;
 }
 __global__ void k_prop_C(const double *P, int ld, int N, int p, int q, const int *old_idx, const double *Phi, double *Cbuf, int ldC) {
+  OVB_PDL_ENTER();
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= N * p)
     return;
@@ -717,6 +725,7 @@ __global__ void k_prop_C(const double *P, int ld, int N, int p, int q, const int
 }
 __global__ void k_prop_PCP(const double *Cbuf, int ldC, int p, int q, const int *old_idx, const double *Phi, const double *Q, double *Sbuf,
                            int ldS) {
+  OVB_PDL_ENTER();
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= p * p)
     return;
@@ -726,6 +735,7 @@ __global__ void k_prop_PCP(const double *Cbuf, int ldC, int p, int q, const int 
 }
 __global__ void k_prop_write(double *P, int ld, int N, int new_off, int p, const double *Cbuf, int ldC, const double *Sbuf, int ldS,
                              DevUpdateInfo *info) {
+  OVB_PDL_ENTER();
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= N * p)
     return;
@@ -746,9 +756,9 @@ void launch_cov_propagate(ovb_ctx *ctx, int new_off, int p, int q, const int *ol
   double *P = ctx->P[ctx->cur];
   int N = ctx->N, ld = ctx->ldP;
   ovb_launch(ctx, k_ekf_prep, dim3(1), dim3(1), (size_t)(0), ctx->d_info, (const int *)nullptr, (const double *)nullptr, 0, 0, 0, (double *)nullptr);
-  k_prop_C<<<(N * p + 255) / 256, 256, 0, ctx->stream>>>(P, ld, N, p, q, old_idx_dev, Phi_dev, ctx->d_M, ld);
-  k_prop_PCP<<<(p * p + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_M, ld, p, q, old_idx_dev, Phi_dev, Q_dev, ctx->d_S, ld);
-  k_prop_write<<<(N * p + 255) / 256, 256, 0, ctx->stream>>>(P, ld, N, new_off, p, ctx->d_M, ld, ctx->d_S, ld, ctx->d_info);
+  ovb_launch(ctx, k_prop_C, dim3((N * p + 255) / 256), dim3(256), (size_t)0, P, ld, N, p, q, old_idx_dev, Phi_dev, ctx->d_M, ld);
+  ovb_launch(ctx, k_prop_PCP, dim3((p * p + 255) / 256), dim3(256), (size_t)0, ctx->d_M, ld, p, q, old_idx_dev, Phi_dev, Q_dev, ctx->d_S, ld);
+  ovb_launch(ctx, k_prop_write, dim3((N * p + 255) / 256), dim3(256), (size_t)0, P, ld, N, new_off, p, ctx->d_M, ld, ctx->d_S, ld, ctx->d_info);
 }
 
 // ovb_marginalize_window: the anchor changes of landmarks l = 0..n-1 (in call order) as one T P T', then the marginalized
@@ -764,6 +774,7 @@ void launch_cov_propagate(ovb_ctx *ctx, int new_off, int p, int q, const int *ol
 __global__ void k_win_rows(int K, int N, const DevWinLM *__restrict__ lms, const int *__restrict__ row_lm, const double *__restrict__ phi,
                            const int *__restrict__ idx, const int *__restrict__ q, const double *__restrict__ P, int ld, double *__restrict__ R,
                            int ldR, const int *flags) {
+  OVB_PDL_ENTER();
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= K * N || flags[1] != 0) // a singular H_f left this landmark without Phi
     return;
@@ -773,6 +784,7 @@ __global__ void k_win_rows(int K, int N, const DevWinLM *__restrict__ lms, const
 __global__ void k_win_blocks(int K, const DevWinLM *__restrict__ lms, const int *__restrict__ row_lm, const double *__restrict__ phi,
                              const int *__restrict__ idx, const int *__restrict__ q, const double *__restrict__ R, int ldR, double *__restrict__ B,
                              int *flags) {
+  OVB_PDL_ENTER();
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= K * K || flags[1] != 0)
     return;
@@ -797,6 +809,7 @@ __global__ void k_win_blocks(int K, const DevWinLM *__restrict__ lms, const int 
 __global__ void k_win_compact(const double *__restrict__ Pin, double *__restrict__ Pout, int ld, int N2, const int *__restrict__ src,
                               const int *__restrict__ mv, const double *__restrict__ R, int ldR, const double *__restrict__ B, int K,
                               const int *__restrict__ flags) {
+  OVB_PDL_ENTER();
   const int i = blockIdx.y * blockDim.y + threadIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N2 || j >= N2 || flags[0] != OVB_NO_NEG_DIAG || flags[1] != 0)
     return;
@@ -821,11 +834,11 @@ void launch_window_shift(ovb_ctx *ctx, int n, int K, int N2, const DevWinLM *lms
   const double *P = ctx->P[ctx->cur];
   const int N = ctx->N, ld = ctx->ldP;
   if (n > 0) {
-    k_win_rows<<<(K * N + 255) / 256, 256, 0, ctx->stream>>>(K, N, lms, row_lm, phi, idx, q, P, ld, R, ldR, flags);
-    k_win_blocks<<<(K * K + 255) / 256, 256, 0, ctx->stream>>>(K, lms, row_lm, phi, idx, q, R, ldR, B, flags);
+    ovb_launch(ctx, k_win_rows, dim3((K * N + 255) / 256), dim3(256), (size_t)0, K, N, lms, row_lm, phi, idx, q, P, ld, R, ldR, flags);
+    ovb_launch(ctx, k_win_blocks, dim3((K * K + 255) / 256), dim3(256), (size_t)0, K, lms, row_lm, phi, idx, q, R, ldR, B, flags);
   }
   dim3 b(32, 8), g((N2 + 31) / 32, (N2 + 7) / 8);
-  k_win_compact<<<g, b, 0, ctx->stream>>>(P, ctx->P[ctx->cur ^ 1], ld, N2, src, mv, R, ldR, B, K, flags);
+  ovb_launch(ctx, k_win_compact, g, b, (size_t)0, P, ctx->P[ctx->cur ^ 1], ld, N2, src, mv, R, ldR, B, K, flags);
 }
 
 // Propagator::propagate_and_clone's accumulation over the IMU steps (Propagator.cpp:83-99, Qd of each step :453-464), in
@@ -852,6 +865,7 @@ __global__ void __launch_bounds__(PA_THREADS) k_prop_accumulate(int n, int steps
   const int tid = threadIdx.x, nn = n * n, rec = nn + 12 * n + 4, npairs = n * (n + 1) / 2;
   double *Phi = pa_sm, *Phi2 = Phi + nn, *Q = Phi2 + nn, *T = Q + nn, *stg = T + nn; // stg: two records [F nn | G 12n | qc 4]
   unsigned char *pi = (unsigned char *)(stg + 2 * rec), *pj = pi + npairs;         // the pairs i <= j, row by row
+  OVB_PDL_ENTER();
   for (int e = tid; e < nn; e += PA_THREADS) {
     Phi[e] = (e / n == e % n) ? 1.0 : 0.0;
     Q[e] = 0.0;
@@ -925,6 +939,5 @@ bool launch_prop_accumulate(ovb_ctx *ctx, int n, int steps, const double *F_dev,
       return false;
     ctx->attr_done[7] = 1;
   }
-  k_prop_accumulate<<<1, PA_THREADS, smem, ctx->stream>>>(n, steps, F_dev, G_dev, qc_dev, Phi_dev, Q_dev);
-  return cudaGetLastError() == cudaSuccess;
+  return ovb_launch(ctx, k_prop_accumulate, dim3(1), dim3(PA_THREADS), smem, n, steps, F_dev, G_dev, qc_dev, Phi_dev, Q_dev) == cudaSuccess;
 }

@@ -1449,7 +1449,6 @@ void launch_feature_system(ovb_ctx *ctx, int n_feats, BlobView bv, int ldH, int 
     ovb_launch(ctx, kern, dim3(grid), dim3(FT_THREADS), smem, ctx->d_frame, ctx->d_opts, ctx->d_feat, L.lo, L.hi, bv, ctx->P[ctx->cur], ctx->ldP,
                ctx->d_chi2_table, ctx->d_Hs, ldH, ovb_feat_order_ptr(ctx), mode, cM, nblk, scratch, per_cta, ctx->d_dump, OVB_MAX_COLS, dump_rows);
     ctx->stream = main_stream;
-    ctx->n_launch++;
   }
   for (int s = 1; s < 3; s++)
     if (used[s]) {
@@ -1483,5 +1482,4 @@ void launch_feature_init(ovb_ctx *ctx, int sched, BlobView bv, int ldH) {
   ovb_launch(ctx, kern, dim3(1), dim3(FT_THREADS), feature_smem_bytes(cM, dm, nblk, path), ctx->d_frame, ctx->d_opts, ctx->d_feat, sched, sched + 1,
              bv, ctx->P[ctx->cur], ctx->ldP, ctx->d_chi2_table, ctx->d_Hs, ldH, nullptr, 0, cM, nblk, scratch, per_cta, (double *)ctx->d_init,
              0, 0);
-  ctx->n_launch++;
 }

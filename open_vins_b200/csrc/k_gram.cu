@@ -25,6 +25,7 @@ __global__ void __launch_bounds__(GR_THREADS) k_gram_partial(const double *__res
                                                              double *__restrict__ Gpart) {
   __shared__ __align__(16) double As[GR_K][GR_T];
   __shared__ __align__(16) double Bs[GR_K][GR_T];
+  OVB_PDL_ENTER();
   // upper tile index -> (ti, tj)
   int t = blockIdx.x, ti = 0;
   while (t >= ntile - ti) {
@@ -84,6 +85,7 @@ __global__ void __launch_bounds__(GR_THREADS) k_gram_partial(const double *__res
 
 // G[i][j] = sum over slabs (fixed order: bitwise reproducible), written for i <= j and mirrored
 __global__ void k_gram_reduce(const double *__restrict__ Gpart, int nslab, int ntile, int ntp, int nt, double *__restrict__ G, int ldG) {
+  OVB_PDL_ENTER();
   const int i = blockIdx.y * 16 + (threadIdx.x >> 4), j = blockIdx.x * 16 + (threadIdx.x & 15);
   if (i >= nt || j >= nt || i > j)
     return;
@@ -108,6 +110,7 @@ __global__ void __launch_bounds__(EKC_THREADS) k_gram_chol(const double *__restr
   extern __shared__ __align__(16) double gsm[];
   __shared__ int flag;
   __shared__ double invd_sh[16];
+  OVB_PDL_ENTER();
   const int tid = threadIdx.x;
   if (tid == 0)
     flag = 0;
@@ -137,7 +140,7 @@ __global__ void __launch_bounds__(EKC_THREADS) k_gram_chol(const double *__restr
 }
 
 // [R | z] (n x (n+1)) <- chol of the Gram of A (m x (n+1), last column = residual). A is not modified.
-int launch_compress_gram(ovb_ctx *ctx, const double *A, int m, int n, int ldA, double *Rout, int ldR) {
+bool launch_compress_gram(ovb_ctx *ctx, const double *A, int m, int n, int ldA, double *Rout, int ldR) {
   const int nt = n + 1;
   const int ntile = (nt + GR_T - 1) / GR_T;
   const int ntp = ntile * (ntile + 1) / 2;
@@ -153,7 +156,7 @@ int launch_compress_gram(ovb_ctx *ctx, const double *A, int m, int n, int ldA, d
       cudaFree(ctx->d_Gpart);
     ctx->d_Gpart = nullptr;
     if (cudaMalloc(&ctx->d_Gpart, sizeof(double) * need_part) != cudaSuccess)
-      return -1;
+      return false;
     ctx->Gpart_cap = need_part;
   }
   if (need_G > ctx->G_cap) {
@@ -161,13 +164,12 @@ int launch_compress_gram(ovb_ctx *ctx, const double *A, int m, int n, int ldA, d
       cudaFree(ctx->d_G);
     ctx->d_G = nullptr;
     if (cudaMalloc(&ctx->d_G, sizeof(double) * need_G) != cudaSuccess)
-      return -1;
+      return false;
     ctx->G_cap = need_G;
   }
-  dim3 g1(ntp, nslab);
-  k_gram_partial<<<g1, GR_THREADS, 0, ctx->stream>>>(A, ldA, m, nt, slab_rows, ntile, ctx->d_Gpart);
-  dim3 g2((nt + 15) / 16, (nt + 15) / 16);
-  k_gram_reduce<<<g2, 256, 0, ctx->stream>>>(ctx->d_Gpart, nslab, ntile, ntp, nt, ctx->d_G, ldG);
+  ovb_launch(ctx, k_gram_partial, dim3(ntp, nslab), dim3(GR_THREADS), (size_t)0, A, ldA, m, nt, slab_rows, ntile, ctx->d_Gpart);
+  ovb_launch(ctx, k_gram_reduce, dim3((nt + 15) / 16, (nt + 15) / 16), dim3(256), (size_t)0, ctx->d_Gpart, nslab, ntile, ntp, nt,
+             ctx->d_G, ldG);
   const size_t smem = sizeof(double) * ((size_t)(n + 1) * (n | 1) + n + 8);
   const int use_smem = smem <= 220 * 1024;
   if (!ctx->attr_done[3]) { // function attributes are per device: one flag per context
@@ -175,7 +177,6 @@ int launch_compress_gram(ovb_ctx *ctx, const double *A, int m, int n, int ldA, d
     ctx->attr_done[3] = 1;
   }
   double *work = ctx->d_G + (size_t)(nt + 2) * ldG;
-  k_gram_chol<<<1, EKC_THREADS, use_smem ? smem : 0, ctx->stream>>>(ctx->d_G, ldG, n, Rout, ldR, work, use_smem);
-  ctx->n_launch += 3;
-  return 3;
+  ovb_launch(ctx, k_gram_chol, dim3(1), dim3(EKC_THREADS), use_smem ? smem : 0, ctx->d_G, ldG, n, Rout, ldR, work, use_smem);
+  return true;
 }

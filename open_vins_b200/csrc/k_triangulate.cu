@@ -30,7 +30,7 @@ __global__ void k_cam_poses(const DevFrame *fr, DevCamPoses *cc) {
 
 void launch_cam_poses(ovb_ctx *ctx) {
   int total = OVB_MAX_CAMS * OVB_MAX_CLONES;
-  k_cam_poses<<<(total + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_frame, ctx->d_cc);
+  ovb_launch(ctx, k_cam_poses, dim3((total + 127) / 128), dim3(128), (size_t)0, ctx->d_frame, ctx->d_cc);
 }
 
 // Sum of one contribution per measurement IN MEASUREMENT ORDER — the order of the reference's loops over

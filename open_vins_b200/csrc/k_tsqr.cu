@@ -634,31 +634,9 @@ void launch_tsqr(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, i
         gy = 1;
       const double *Win = level > 0 ? ctx->d_W[(level - 1) & 1] : nullptr;
       double *Wout = ctx->d_W[level & 1];
-      {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(gx, gy);
-        cfg.blockDim = dim3(QR_THREADS);
-        cfg.dynamicSmemBytes = sizeof(QrSmem);
-        cfg.stream = ctx->stream;
-        cudaLaunchAttribute at[2];
-        int na = 0;
-        if (ctx->tsqr_pdl) { // overlap this kernel's launch + prologue with the tail of the previous one
-          at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-          at[na].val.programmaticStreamSerializationAllowed = 1;
-          na++;
-        }
-        if (clustered) {
-          at[na].id = cudaLaunchAttributeClusterDimension;
-          at[na].val.clusterDim.x = QR_CLUSTER;
-          at[na].val.clusterDim.y = 1;
-          at[na].val.clusterDim.z = 1;
-          na++;
-        }
-        cfg.attrs = at;
-        cfg.numAttrs = na;
-        cudaLaunchKernelEx(&cfg, k_tsqr_level, A, ldA, nt, c0, nbp, level, len, Win, Wout, Rout, ldR, last, clustered ? (int)QR_CLUSTER : 1, cr0);
-      }
-      ctx->n_launch++;
+      const int cl = clustered ? QR_CLUSTER : 1;
+      ovb_launch(ctx, k_tsqr_level, ovb_grid(dim3(gx, gy), dim3(cl)), dim3(QR_THREADS), sizeof(QrSmem), A, ldA, nt, c0, nbp, level, len, Win, Wout, Rout,
+                 ldR, last, cl, cr0);
       ctx->n_launch_tsqr_level++;
       if (last)
         break;
@@ -668,7 +646,6 @@ void launch_tsqr(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, i
     }
   }
   ovb_launch(ctx, k_tsqr_assemble, dim3(n), dim3(128), (size_t)(0), A, ldA, m, n, Rout, ldR);
-  ctx->n_launch++;
 }
 
 // =====================================================================================================================
@@ -681,6 +658,7 @@ __global__ void k_column_map(const DevFrame *__restrict__ fr, const DevOpts *__r
   __shared__ int n_used_feats, rows_stacked;
   __shared__ int order[OVB_MAX_VARS];
   __shared__ int n_order;
+  OVB_PDL_ENTER();
   const int tid = threadIdx.x;
   if (tid < OVB_MAX_VARS)
     key[tid] = 0xffffffffu;
@@ -754,7 +732,8 @@ __global__ void k_column_map(const DevFrame *__restrict__ fr, const DevOpts *__r
 }
 
 void launch_column_map(ovb_ctx *ctx, int n_feats, BlobView bv, int rows_drop) {
-  k_column_map<<<1, 256, 0, ctx->stream>>>(ctx->d_frame, ctx->d_opts, ctx->d_feat, n_feats, ovb_feat_order_ptr(ctx), ctx->d_info, rows_drop);
+  ovb_launch(ctx, k_column_map, dim3(1), dim3(256), (size_t)0, ctx->d_frame, ctx->d_opts, ctx->d_feat, n_feats, ovb_feat_order_ptr(ctx), ctx->d_info,
+             rows_drop);
 }
 
 // SLAM update: the variables are the frame's slots plus one landmark per feature. A feature's landmark is the last entry of
@@ -772,6 +751,7 @@ __global__ void k_column_map_slam(const DevFrame *__restrict__ fr, const DevOpts
   __shared__ unsigned int ekey[CM_MAX_ENT];
   __shared__ int order[CM_MAX_ENT];
   __shared__ int n_used_feats, rows_stacked, lm_cols;
+  OVB_PDL_ENTER();
   const int tid = threadIdx.x;
   if (tid < OVB_MAX_VARS)
     key[tid] = 0xffffffffu;
@@ -879,8 +859,8 @@ __global__ void k_column_map_slam(const DevFrame *__restrict__ fr, const DevOpts
 }
 
 void launch_column_map_slam(ovb_ctx *ctx, int n_feats, bool full_map) {
-  k_column_map_slam<<<1, 256, 0, ctx->stream>>>(ctx->d_frame, ctx->d_opts, ctx->d_feat, n_feats, ovb_feat_order_ptr(ctx), ctx->d_info,
-                                                full_map ? 1 : 0);
+  ovb_launch(ctx, k_column_map_slam, dim3(1), dim3(256), (size_t)0, ctx->d_frame, ctx->d_opts, ctx->d_feat, n_feats, ovb_feat_order_ptr(ctx),
+             ctx->d_info, full_map ? 1 : 0);
 }
 
 // B[i][q] = Rin[i][col_canon[q]] for q < n_all, B[i][n_all] = Rin[i][n_all] (residual)
@@ -898,6 +878,5 @@ void launch_reorder_R(ovb_ctx *ctx, const double *Rin, int n_all, int ldRin, dou
   // permuted copy into the (now free) staging matrix, then the same TSQR re-triangularises it
   int ldB = ldRin;
   ovb_launch(ctx, k_gather_cols, dim3(n_all), dim3(128), (size_t)(0), Rin, ldRin, n_all, ctx->d_info, ctx->d_Hs, ldB);
-  ctx->n_launch++;
   launch_tsqr(ctx, ctx->d_Hs, n_all, n_all, ldB, Rout, ldRout);
 }

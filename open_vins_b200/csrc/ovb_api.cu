@@ -18,9 +18,43 @@ unsigned char *ovb_feat_order_ptr(ovb_ctx *ctx) { return ctx->d_feat_order; }
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+int ovb_prof_slot(ovb_ctx *ctx, const void *kern) {
+  if (ctx->prof_n == ctx->prof_cap) { // grow the pool: twice the pairs, created one pair at a time
+    const int cap = ctx->prof_cap ? 2 * ctx->prof_cap : 128;
+    cudaEvent_t *ev = (cudaEvent_t *)realloc(ctx->prof_ev, sizeof(cudaEvent_t) * 2 * cap);
+    if (ev)
+      ctx->prof_ev = ev;
+    const void **fn = (const void **)realloc(ctx->prof_fn, sizeof(const void *) * cap);
+    if (fn)
+      ctx->prof_fn = fn;
+    for (; ev && fn && ctx->prof_cap < cap; ctx->prof_cap++) {
+      cudaEvent_t *pair = ctx->prof_ev + 2 * ctx->prof_cap;
+      pair[0] = pair[1] = nullptr;
+      if (cudaEventCreate(&pair[0]) != cudaSuccess || cudaEventCreate(&pair[1]) != cudaSuccess) {
+        cudaGetLastError();
+        if (pair[0]) // the first of the pair was created
+          cudaEventDestroy(pair[0]);
+        break;
+      }
+    }
+    if (ctx->prof_n == ctx->prof_cap)
+      return -1; // out of memory: this launch is not profiled
+  }
+  ctx->prof_fn[ctx->prof_n] = kern;
+  return ctx->prof_n++;
+}
+
 extern "C" {
 
 static ovb_status ensure_stage(ovb_ctx *ctx, size_t doubles);
+
+// Every entry point that launches kernels starts here, so that ovb_last_counters and ovb_profile_read describe its
+// launches alone (ovb_msckf_shard_finish continues the count of its ovb_msckf_shard_compress).
+static void begin_launches(ovb_ctx *ctx) {
+  ctx->n_launch = 0;
+  ctx->n_launch_tsqr_level = 0;
+  ctx->prof_n = 0;
+}
 
 int ovb_abi_version(void) { return OVB_ABI_VERSION; }
 
@@ -96,7 +130,7 @@ ovb_status ovb_create(const ovb_config *cfg, ovb_ctx **out) {
     const char *e = getenv("OVB_TSQR_CLUSTER");
     ctx->tsqr_cluster = e ? atoi(e) : 1;
     const char *e2 = getenv("OVB_TSQR_PDL");
-    ctx->tsqr_pdl = e2 ? atoi(e2) : 1;
+    ctx->pdl = e2 ? atoi(e2) : 1;
     const char *e3 = getenv("OVB_FEAT_CLASSES");
     ctx->feat_classes = e3 ? atoi(e3) : 1;
     const char *e4 = getenv("OVB_EKF_CHOL_DMMA");
@@ -183,15 +217,15 @@ ovb_status ovb_create(const ovb_config *cfg, ovb_ctx **out) {
 }
 
 void ovb_destroy(ovb_ctx *ctx) {
-  if (ctx)
-    for (int i = 0; i < 2 * 96; i++)
-      if (ctx->prof_ev[i])
-        cudaEventDestroy(ctx->prof_ev[i]);
   if (!ctx)
     return;
   cudaSetDevice(ctx->device);
   if (ctx->stream)
     cudaStreamSynchronize(ctx->stream);
+  for (int i = 0; i < 2 * ctx->prof_cap; i++)
+    cudaEventDestroy(ctx->prof_ev[i]);
+  free(ctx->prof_ev);
+  free(ctx->prof_fn);
   void *dev[] = {ctx->P[0],   ctx->P[1], ctx->d_arena, ctx->d_cc, ctx->d_feat_order, ctx->d_info, ctx->d_chi2_table, ctx->d_Hs, ctx->d_W[0],
                  ctx->d_W[1], ctx->d_R,  ctx->d_R2,    ctx->d_M,  ctx->d_S,          ctx->d_Y,    ctx->d_w,          ctx->d_scratch,
                  ctx->d_long, ctx->d_dump, ctx->P_snap, ctx->d_flush, ctx->d_Gpart, ctx->d_G, ctx->d_cqw, ctx->d_grp, ctx->d_grp_acc, ctx->d_init, ctx->d_imu, ctx->d_pub};
@@ -284,6 +318,7 @@ ovb_status ovb_cov_clone(ovb_ctx *ctx, int old_off, int size, const double *dnc_
   if (dnc_dt && (dt_off < 0 || dt_off >= ctx->N || size > 64))
     return OVB_ERR_ARG;
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   const double *dnc_dev = nullptr;
   if (dnc_dt) {
     memcpy(ctx->h_dx, dnc_dt, sizeof(double) * size);
@@ -301,6 +336,7 @@ ovb_status ovb_cov_marginalize(ovb_ctx *ctx, int off, int size) {
   if (!ctx || size < 1 || off < 0 || off + size > ctx->N)
     return OVB_ERR_ARG;
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   launch_cov_marginalize(ctx, off, size);
   OVB_CUDA_CHECK(ctx, cudaGetLastError());
   OVB_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
@@ -387,6 +423,7 @@ ovb_status ovb_marginalize_window(ovb_ctx *ctx, const ovb_frame *fr, const ovb_o
     return OVB_ERR_CAPACITY;
   }
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   {
     ovb_status es = ensure_stage(ctx, total / sizeof(double) + 1);
     if (es != OVB_OK)
@@ -498,6 +535,7 @@ ovb_status ovb_cov_propagate(ovb_ctx *ctx, int new_off, int p, const int *old_of
     return OVB_ERR_CAPACITY;
   }
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   // stage: [Phi p*q][Q p*p] doubles, then q ints
   {
     ovb_status es = ensure_stage(ctx, (size_t)p * q + (size_t)p * p + (size_t)q + 16);
@@ -557,6 +595,7 @@ ovb_status ovb_cov_propagate_imu(ovb_ctx *ctx, int n, int steps, const double *F
   if (2 * nn > ctx->Hs_cap)
     return OVB_ERR_CAPACITY;
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   // staging (doubles): [F steps*nn][G steps*12n][qc steps*4][dnc_dt clone_size][old indices n ints]; Phi, Q come back in front
   const size_t oF = 0, oG = oF + (size_t)steps * nn, oq = oG + (size_t)steps * 12 * n, od = oq + (size_t)steps * 4,
                oi = od + (dnc_dt ? (size_t)clone_size : 0), in_doubles = oi + ((size_t)n + 1) / 2;
@@ -1087,6 +1126,7 @@ ovb_status ovb_triangulate(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat_
   if (!ctx || !out)
     return OVB_ERR_ARG;
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   Packed pk;
   int saveN = ctx->N;
   if (ctx->N == 0)
@@ -1114,6 +1154,7 @@ ovb_status ovb_feature_jacobians(ovb_ctx *ctx, const ovb_frame *frame, const ovb
     return OVB_ERR_ARG;
   }
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   Packed pk;
   ovb_status st = pack_inputs(ctx, frame, feats, opts, out, &pk);
   if (st != OVB_OK)
@@ -1242,6 +1283,7 @@ ovb_status ovb_slam_delayed_init_reps(ovb_ctx *ctx, const ovb_frame *frame, cons
   int64_t *cnt = ctx->init_counters; // features processed, stream synchronisations, bytes H2D, bytes D2H
   cnt[0] = cnt[1] = cnt[2] = cnt[3] = 0;
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   // 1. pack and upload the batch once; triangulate + GN all tracks at the current state (UpdaterSLAM.cpp:118-142). The
   // tracks' anchors and positions stay on the device for the per-feature systems.
   Packed pk;
@@ -1388,6 +1430,7 @@ ovb_status ovb_last_init_counters(const ovb_ctx *ctx, int64_t out[4]) {
 
 // dx = 0 when no row reaches the EKF update
 __global__ void k_fill_zero_dx(double *dx, int N) {
+  OVB_PDL_ENTER();
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < N)
     dx[i] = 0.0;
@@ -1444,9 +1487,9 @@ __global__ void k_group_finish(double *__restrict__ P, int ldP, int N, const dou
 // measurement_compress_inplace in the requested mode; returns the number of rows of [R | z] handed to the EKF update.
 // The Cholesky-based modes always produce n rows; the Householder path leaves min(m, n).
 static int compress_system(ovb_ctx *ctx, int mode, double *A, int m, int n, int ldA, double *Rout, int ldR) {
-  if (mode == OVB_COMPRESS_CHOLQR2 && launch_compress_cholqr2(ctx, A, m, n, ldA, Rout, ldR) >= 0)
+  if (mode == OVB_COMPRESS_CHOLQR2 && launch_compress_cholqr2(ctx, A, m, n, ldA, Rout, ldR))
     return n;
-  if (mode == OVB_COMPRESS_NORMAL_EQUATIONS && launch_compress_gram(ctx, A, m, n, ldA, Rout, ldR) >= 0)
+  if (mode == OVB_COMPRESS_NORMAL_EQUATIONS && launch_compress_gram(ctx, A, m, n, ldA, Rout, ldR))
     return n;
   launch_tsqr(ctx, A, m, n, ldA, Rout, ldR);
   return std::min(m, n);
@@ -1462,15 +1505,10 @@ static int enqueue_slam_groups(ovb_ctx *ctx, int n_groups, int ldH);
 static int enqueue_update(ovb_ctx *ctx, const Packed &pk, int col_order, cudaEvent_t *ev, bool slam = false) {
   const int N = ctx->N, F = pk.n_feats, ldH = pk.ldH, m_total = pk.m_total, n_all = pk.n_all, n_groups = pk.n_groups;
   const BlobView bv = pk.bv;
-  ctx->n_launch = 0;
-  ctx->n_launch_tsqr_level = 0;
-  ctx->prof_n = 0;
   if (!slam) {
     launch_cam_poses(ctx);
     launch_triangulate(ctx, F, bv);
-    ctx->n_launch += 2;
   }
-  ctx->n_launch += 1; // column map (the per-feature kernel counts its own launches: one, or one per size class)
   if (ev)
     cudaEventRecord(ev[1], ctx->stream);
   launch_feature_system(ctx, F, bv, ldH, slam ? 2 : 0);
@@ -1517,13 +1555,10 @@ static int enqueue_update(ovb_ctx *ctx, const Packed &pk, int col_order, cudaEve
     cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0);
   if (ev)
     cudaEventRecord(ev[4], ctx->stream);
-  if (r > 0) {
+  if (r > 0)
     launch_ekf_update(ctx, Rfinal, ldR, r, n_all, false, slam ? 1.0 : ctx->h_opts->sigma_pix_sq, nullptr);
-    ctx->n_launch += 6; // prep, 2 gemm, chol, trsm, downdate
-  } else {
-    k_fill_zero_dx<<<(N + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_dx, N);
-    ctx->n_launch += 1;
-  }
+  else
+    ovb_launch(ctx, k_fill_zero_dx, dim3((N + 127) / 128), dim3(128), (size_t)0, ctx->d_dx, N);
   if (ev)
     cudaEventRecord(ev[5], ctx->stream);
   return r;
@@ -1548,42 +1583,35 @@ static int enqueue_slam_groups(ovb_ctx *ctx, int n_groups, int ldH) {
     launch_ekf_update(ctx, ctx->d_R, ldH, r, n, false, 1.0, nullptr);
     ovb_launch(ctx, k_group_accumulate, dim3((N + 255) / 256), dim3(256), (size_t)0, (const double *)ctx->d_dx, acc, N,
                (const DevUpdateInfo *)ctx->d_info, flags);
-    ctx->n_launch += 8; // group_take_z, prep, 2 gemm, chol, trsm, downdate, accumulate
     r_total += r;
   }
-  if (r_total > 0) {
+  if (r_total > 0)
     ovb_launch(ctx, k_group_finish, dim3((N + 31) / 32, (N + 7) / 8), dim3(32, 8), (size_t)0, P, ld, N, (const double *)ctx->P_snap,
                (const double *)acc, ctx->d_dx, ctx->d_info, (const int *)flags);
-  } else {
-    k_fill_zero_dx<<<(N + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_dx, N);
-  }
-  ctx->n_launch += 1;
+  else
+    ovb_launch(ctx, k_fill_zero_dx, dim3((N + 127) / 128), dim3(128), (size_t)0, ctx->d_dx, N);
   return r_total;
 }
 
-// Per-kernel timing of the update pipeline (bench.py's roofline block): while on, every kernel launched through
-// ovb_launch on the context stream is bracketed by CUDA events and programmatic dependent launch is disabled, so each
-// duration is that kernel alone, in stream order, with whatever the previous kernels left in L2.
+// Per-kernel timing (bench.py's roofline block): while on, every kernel launched through ovb_launch is bracketed by CUDA
+// events and programmatic dependent launch is disabled, so each duration is that kernel alone, in stream order, with
+// whatever the previous kernels left in L2.
 ovb_status ovb_set_profile(ovb_ctx *ctx, int enabled) {
   if (!ctx)
     return OVB_ERR_ARG;
-  OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-  if (enabled && ctx->prof_ev[0] == nullptr)
-    for (int i = 0; i < 2 * 96; i++)
-      OVB_CUDA_CHECK(ctx, cudaEventCreate(&ctx->prof_ev[i]));
   ctx->prof_on = enabled ? 1 : 0;
   ctx->prof_n = 0;
   return OVB_OK;
 }
 
-// kernels of the LAST update call, in launch order: names (NUL-separated, truncated to name_cap bytes in total) and their
-// durations in microseconds. *n = number of entries (<= cap). Call after the update returned (the stream is idle).
+// kernels of the last call, in launch order: names (NUL-separated, truncated to name_cap bytes in total) and their
+// durations in microseconds, min(cap, *n) of them, where *n = the call's launches. Call after the call returned.
 ovb_status ovb_profile_read(ovb_ctx *ctx, char *names, int name_cap, float *us, int cap, int *n) {
   if (!ctx || !names || !us || !n || name_cap < 1)
     return OVB_ERR_ARG;
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-  int w = 0, k = 0;
-  for (; k < ctx->prof_n && k < cap; k++) {
+  int w = 0;
+  for (int k = 0; k < ctx->prof_n && k < cap; k++) {
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, ctx->prof_ev[2 * k], ctx->prof_ev[2 * k + 1]) != cudaSuccess)
       cudaGetLastError();
@@ -1599,7 +1627,7 @@ ovb_status ovb_profile_read(ovb_ctx *ctx, char *names, int name_cap, float *us, 
   }
   if (w < name_cap)
     names[w] = 0;
-  *n = k;
+  *n = ctx->prof_n;
   return OVB_OK;
 }
 
@@ -1614,7 +1642,7 @@ ovb_status ovb_last_host_us(const ovb_ctx *ctx, double out[4]) {
 ovb_status ovb_last_counters(const ovb_ctx *ctx, int64_t out[4]) {
   if (!ctx || !out)
     return OVB_ERR_ARG;
-  out[0] = ctx->n_launch;            // kernels launched by the last update pipeline
+  out[0] = ctx->n_launch;            // kernels launched by the last call
   out[1] = ctx->n_launch_tsqr_level; // of which k_tsqr_level
   out[2] = (int64_t)ctx->last_h2d_bytes;
   out[3] = (int64_t)ctx->last_d2h_bytes;
@@ -1650,6 +1678,7 @@ ovb_status ovb_msckf_replay(ovb_ctx *ctx, int steps, int flush_l2, float *ms_per
   const size_t flush_bytes = (size_t)256 << 20; // five times the 50 MB L2 of an H100
   if (flush_l2 && !ctx->d_flush)
     OVB_CUDA_CHECK(ctx, cudaMalloc(&ctx->d_flush, flush_bytes));
+  begin_launches(ctx);
   std::vector<cudaEvent_t> evs((size_t)steps * 6);
   for (auto &e : evs)
     OVB_CUDA_CHECK(ctx, cudaEventCreate(&e));
@@ -1699,6 +1728,7 @@ ovb_status ovb_msckf_update(ovb_ctx *ctx, const ovb_frame *frame, const ovb_feat
   }
   for (int i = 0; i < N; i++)
     dx[i] = 0.0;
+  begin_launches(ctx);
   if (!feats || feats->n_feats <= 0) // UpdaterMSCKF.cpp:61-62
     return OVB_OK;
   cudaEventRecord(ctx->ev[0], ctx->stream);
@@ -1763,6 +1793,7 @@ ovb_status ovb_slam_update_reps(ovb_ctx *ctx, const ovb_frame *frame, const ovb_
   }
   for (int i = 0; i < N; i++)
     dx[i] = 0.0;
+  begin_launches(ctx);
   if (!feats || feats->n_feats <= 0) // UpdaterSLAM.cpp:256-257
     return OVB_OK;
   cudaEventRecord(ctx->ev[0], ctx->stream);
@@ -1884,6 +1915,7 @@ ovb_status ovb_msckf_shard_compress(ovb_ctx *ctx, const ovb_frame *frame, const 
   if (!ctx || !frame || !feats || !opts || !R_dev || !n_cols || !ld || ctx->N < 1)
     return OVB_ERR_ARG;
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   cudaEventRecord(ctx->ev[0], ctx->stream);
   Packed pk;
   ovb_opts o2 = *opts;
@@ -1897,13 +1929,10 @@ ovb_status ovb_msckf_shard_compress(ovb_ctx *ctx, const ovb_frame *frame, const 
   if ((size_t)pk.n_all * pk.ldH > (size_t)R_cap_doubles)
     return OVB_ERR_CAPACITY;
   ctx->last_pk = pk;
-  ctx->n_launch = 0;
-  ctx->n_launch_tsqr_level = 0;
   launch_cam_poses(ctx);
   launch_triangulate(ctx, pk.n_feats, pk.bv);
   launch_feature_system(ctx, pk.n_feats, pk.bv, pk.ldH, 0);
   launch_column_map(ctx, pk.n_feats, pk.bv);
-  ctx->n_launch += 3; // cam poses, triangulate, column map (+ the per-feature kernel's own count)
   if (pk.m_total > 0)
     compress_system(ctx, o2.compress, ctx->d_Hs, pk.m_total, pk.n_all, pk.ldH, R_dev, pk.ldH); // unused rows of the block read as zero
   else
@@ -1924,7 +1953,6 @@ ovb_status ovb_msckf_shard_finish(ovb_ctx *ctx, double *stacked_dev, int n_block
     Rfinal = ctx->d_R;
   }
   launch_ekf_update(ctx, Rfinal, ld, n_all, n_all, false, ctx->h_opts->sigma_pix_sq, nullptr);
-  ctx->n_launch += 6; // prep, 2 gemm, chol, trsm, downdate
   cudaEventRecord(ctx->ev[5], ctx->stream);
   ovb_status st = enqueue_readback(ctx, F);
   if (st != OVB_OK)
@@ -1961,6 +1989,7 @@ ovb_status ovb_msckf_shard_finish(ovb_ctx *ctx, double *stacked_dev, int n_block
 // ------------------------------------------------------------------------------------------------ staged dense entry points
 // rows scaled by 1/sqrt(Rdiag): whitening turns R = diag(Rdiag) into the identity so that compression applies
 __global__ void k_whiten_rows(double *A, int ld, int m, int ncols) {
+  OVB_PDL_ENTER();
   int i = blockIdx.x;
   double s = 1.0 / sqrt(A[(size_t)i * ld + ncols]); // the row's noise variance rides in column ncols
   __syncthreads();
@@ -2012,6 +2041,7 @@ static ovb_status compress_dense(ovb_ctx *ctx, int mode, const double *H, int m,
   if (n > ctx->cfg.max_state)
     return OVB_ERR_CAPACITY;
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   int ld;
   ovb_status st = stage_dense(ctx, H, m, n, res, nullptr, &ld);
   if (st != OVB_OK)
@@ -2019,9 +2049,9 @@ static ovb_status compress_dense(ovb_ctx *ctx, int mode, const double *H, int m,
   if (mode == OVB_COMPRESS_HOUSEHOLDER_TSQR) {
     launch_tsqr(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld);
   } else if (mode == OVB_COMPRESS_NORMAL_EQUATIONS) {
-    if (launch_compress_gram(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld) < 0)
+    if (!launch_compress_gram(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld))
       return OVB_ERR_CUDA;
-  } else if (launch_compress_cholqr2(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld) < 0) {
+  } else if (!launch_compress_cholqr2(ctx, ctx->d_Hs, m, n, ld, ctx->d_R, ld)) {
     snprintf(ctx->err, sizeof(ctx->err), "ovb_compress_cholqr2: %d columns exceed what this path takes", n);
     return OVB_ERR_CAPACITY;
   }
@@ -2065,6 +2095,7 @@ ovb_status ovb_ekf_update(ovb_ctx *ctx, const int *off, const int *sz, int nvar,
   if (n > OVB_MAX_COLS || n > ctx->cfg.max_state)
     return OVB_ERR_CAPACITY;
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   if (Rdiag)
     for (int i = 0; i < r; i++)
       if (!(Rdiag[i] > 0.0))
@@ -2085,7 +2116,7 @@ ovb_status ovb_ekf_update(ovb_ctx *ctx, const int *off, const int *sz, int nvar,
   double s2 = sigma2;
   if (Rdiag) {
     // whiten each row by 1/sqrt(R_ii) so that R = I; then compression is admissible (UpdaterSLAM.cpp:444 uses diagonal R)
-    k_whiten_rows<<<r, 128, 0, ctx->stream>>>(ctx->d_Hs, ld, r, n + 1);
+    ovb_launch(ctx, k_whiten_rows, dim3(r), dim3(128), (size_t)0, ctx->d_Hs, ld, r, n + 1);
     s2 = 1.0;
   }
   if (r > n) {
@@ -2125,6 +2156,7 @@ ovb_status ovb_cov_initialize(ovb_ctx *ctx, const int *off, const int *sz, int n
     return OVB_ERR_CAPACITY;
   }
   OVB_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+  begin_launches(ctx);
   *accepted = 0;
   // ---- Givens split (StateHelper.cpp:429-440), row-major copies
   std::vector<double> HR(H_R_in, H_R_in + (size_t)r * n), HL(H_L_in, H_L_in + (size_t)r * k), res(res_in, res_in + r);

@@ -215,7 +215,7 @@ struct ovb_ctx {
   int sm_count;
   size_t info_bytes; // DevUpdateInfo rounded up: d_dx / h_dx start right behind d_info / h_info
   int attr_done[9]; // per-context (= per-device) one-time cudaFuncSetAttribute flags: 0 tsqr, 1 feature, 2 ekf, 3 gram, 4 cholqr, 8 triangulate
-  int tsqr_pdl;     // programmatic dependent launch between the TSQR level kernels (OVB_TSQR_PDL=0 disables: A/B timing only)
+  int pdl;          // programmatic dependent launch on every ovb_launch (OVB_TSQR_PDL=0 disables: A/B timing only)
   int tsqr_cluster; // upper TSQR levels as one thread-block cluster (OVB_TSQR_CLUSTER=0 disables: A/B timing only)
   int gram_cluster;  // k_cq_gram: clusters of 4 slabs pre-reduce in distributed shared memory (OVB_GRAM_CLUSTER=0 disables: A/B timing only)
   int ekf_chol_dmma; // EKF Cholesky on the DMMA kernel of k_cholqr.cu (OVB_EKF_CHOL_DMMA=0 disables: A/B timing only)
@@ -235,7 +235,7 @@ struct ovb_ctx {
   int grp_cap;
   double *d_grp_acc;
   int slam_unbounded; // ovb_set_slam_unbounded: SLAM batches beyond OVB_MAX_VARS variables (else OVB_ERR_CAPACITY, as before)
-  // bookkeeping for bench.py: kernels launched by the last update pipeline, bytes moved by the last ovb_msckf_update
+  // bookkeeping for bench.py: kernels launched by the last call (counted by ovb_launch), bytes moved by the last ovb_msckf_update
   int n_launch, n_launch_tsqr_level;
   // normal-equations compression (k_gram.cu)
   double *d_Gpart, *d_G;
@@ -254,10 +254,11 @@ struct ovb_ctx {
   // side also receives Phi and Q. Reserved at ovb_create for ordinary frames, grown with headroom beyond.
   double *d_imu, *h_imu;
   size_t imu_cap; // doubles
-  // per-kernel profile (ovb_set_profile): CUDA events around every ovb_launch of the main stream; PDL is off while it is on
-  int prof_on, prof_n;
-  cudaEvent_t prof_ev[2 * 96];
-  const void *prof_fn[96];
+  // per-kernel profile (ovb_set_profile): CUDA events around every ovb_launch of the last call; PDL is off while it is on.
+  // The pool of prof_cap event pairs grows on demand (ovb_prof_slot).
+  int prof_on, prof_n, prof_cap;
+  cudaEvent_t *prof_ev; // [2 * prof_cap]
+  const void **prof_fn; // [prof_cap]
 };
 
 #define OVB_CUDA_CHECK(ctx, call)                                                                                     \
@@ -292,11 +293,11 @@ void launch_column_map_slam(ovb_ctx *ctx, int n_feats, bool full_map);
 // TSQR of A [m x (n+1)] (last column = residual) in place; R (n x (n+1), diag>=0) to Rout with leading dimension ldR
 void launch_tsqr(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR);
 // gather columns of Rin in the order info->col_canon (n_used of them) into Hs scratch and re-triangularise into Rout
-// [R | z] <- chol([H r]'[H r]) (k_gram.cu); returns the number of kernels launched or -1
-int launch_compress_gram(ovb_ctx *ctx, const double *A, int m, int n, int ldA, double *Rout, int ldR);
+// [R | z] <- chol([H r]'[H r]) (k_gram.cu); false when its buffers could not be allocated
+bool launch_compress_gram(ovb_ctx *ctx, const double *A, int m, int n, int ldA, double *Rout, int ldR);
 // [R | z] <- shifted CholeskyQR2 of A (k_cholqr.cu; A is kept up to CQ_MAXN columns, overwritten by the wider blocked
-// path); returns kernels launched, or -1 when the system is too wide for it (callers then use launch_tsqr)
-int launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR);
+// path); false when the system is too wide for it (callers then use launch_tsqr)
+bool launch_compress_cholqr2(ovb_ctx *ctx, double *A, int m, int n, int ldA, double *Rout, int ldR);
 // EKF Cholesky on the DMMA kernel of k_cholqr.cu; false when r does not fit (caller uses k_ekf_chol)
 // epoch_out != nullptr: the factor streams to the launch_trsm_rows that follows (epoch 0: it does not)
 bool launch_chol_ekf_dmma(ovb_ctx *ctx, double *S, int ldS, int r, const double *res, double *w, double *invdiag, double **Lpk_out,
@@ -336,37 +337,59 @@ bool launch_prop_accumulate(ovb_ctx *ctx, int n, int steps, const double *F_dev,
                             double *Q_dev);
 
 // ---- programmatic dependent launch (PDL) ----------------------------------------------------------------------------
-// Every kernel of the update pipeline starts with OVB_PDL_ENTER(): it lets the NEXT kernel of the stream be scheduled
-// while this one runs (its CTAs become resident on idle SMs and block), then waits until the PREVIOUS kernel has
-// completed and flushed. Semantics are those of ordinary stream order; what is saved is the launch latency between the
-// ~30 dependent, latency-bound kernels of one update. Both instructions are no-ops in a kernel launched without the
-// attribute. ovb_launch() adds the attribute when ctx->tsqr_pdl is set (OVB_TSQR_PDL=0 disables it).
+// Every kernel starts with OVB_PDL_ENTER() (or places the two instructions itself): it lets the NEXT kernel of the
+// stream be scheduled while this one runs (its CTAs become resident on idle SMs and block), then waits until the
+// PREVIOUS kernel has completed and flushed. Semantics are those of ordinary stream order as long as nothing before the
+// wait touches memory another kernel writes; what is saved is the launch latency between the dependent, latency-bound
+// kernels of one call. Both instructions are no-ops in a kernel launched without the attribute.
 #define OVB_PDL_ENTER()                                                     \
   do {                                                                      \
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");         \
     asm volatile("griddepcontrol.wait;" ::: "memory");                      \
   } while (0)
 
+// the profile slot of the next launch of kern (the pool grows as needed), or -1 when no event could be created
+int ovb_prof_slot(ovb_ctx *ctx, const void *kern);
+
+// launch geometry: the grid, optionally as thread-block clusters of `cluster` CTAs
+struct ovb_grid {
+  dim3 blocks, cluster;
+  ovb_grid(dim3 b, dim3 c = dim3(1, 1, 1)) : blocks(b), cluster(c) {}
+};
+
 #ifdef __CUDACC__
+// The one launch site of the library: enqueues kern on ctx->stream with the PDL attribute when ctx->pdl is set and
+// profiling is off, counts the launch in ctx->n_launch and, while profiling, brackets it with a pair of CUDA events.
 template <typename... KArgs, typename... Args>
-static inline void ovb_launch(ovb_ctx *ctx, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, Args &&...args) {
+static inline cudaError_t ovb_launch(ovb_ctx *ctx, void (*kern)(KArgs...), ovb_grid grid, dim3 block, size_t smem, Args &&...args) {
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
+  cfg.gridDim = grid.blocks;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = ctx->stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = (ctx->tsqr_pdl && !ctx->prof_on) ? 1 : 0;
-  const bool prof = ctx->prof_on && ctx->prof_n < 96 && ctx->prof_ev[0] != nullptr;
-  if (prof)
-    cudaEventRecord(ctx->prof_ev[2 * ctx->prof_n], ctx->stream);
-  cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-  if (prof) {
-    cudaEventRecord(ctx->prof_ev[2 * ctx->prof_n + 1], ctx->stream);
-    ctx->prof_fn[ctx->prof_n++] = (const void *)kern;
+  cudaLaunchAttribute at[2];
+  int na = 0;
+  if (ctx->pdl && !ctx->prof_on) {
+    at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[na].val.programmaticStreamSerializationAllowed = 1;
+    na++;
   }
+  if (grid.cluster.x * grid.cluster.y * grid.cluster.z > 1) {
+    at[na].id = cudaLaunchAttributeClusterDimension;
+    at[na].val.clusterDim.x = grid.cluster.x;
+    at[na].val.clusterDim.y = grid.cluster.y;
+    at[na].val.clusterDim.z = grid.cluster.z;
+    na++;
+  }
+  cfg.attrs = at;
+  cfg.numAttrs = na;
+  const int slot = ctx->prof_on ? ovb_prof_slot(ctx, (const void *)kern) : -1;
+  if (slot >= 0)
+    cudaEventRecord(ctx->prof_ev[2 * slot], ctx->stream);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+  if (slot >= 0)
+    cudaEventRecord(ctx->prof_ev[2 * slot + 1], ctx->stream);
+  ctx->n_launch++;
+  return e;
 }
 #endif
