@@ -24,7 +24,10 @@ CASE_CONFIG2 = os.path.join(os.path.dirname(HERE), "tests", "golden", "rpng_sim_
 
 def run(exe=None, traj=None, cams=2, clones=11, msckf=10, pts=250, frames=0, calib=1, est=None, timing=None, capture=None, integration="rk4",
         compress="cholqr2", seed_init=0, seed_perturb=0, seed_meas=0, runs=None, jobs=None, out_dir=None, consistency=None, cam_model=None,
-        slam=None, slam_in_update=None, slam_delay=None, feat_rep_slam=None, slam_log=None, perturb=False, timeout=1800):
+        slam=None, slam_in_update=None, slam_delay=None, feat_rep_slam=None, slam_log=None, perturb=False, feat_rep_msckf=None, use_fej=None,
+        fi_triangulate_1d=None, fi_refine_features=None, up_msckf_sigma_px=None, up_msckf_chi2_multipler=None, up_slam_sigma_px=None,
+        up_slam_chi2_multipler=None, calib_cam_extrinsics=None, calib_cam_intrinsics=None, calib_cam_timeoffset=None, calib_imu_intrinsics=None,
+        calib_imu_g_sensitivity=None, timeout=1800):
     """Runs the simulation; returns the parsed JSON summary. capture = (frame_index, path_prefix) dumps that update's inputs.
     seed_init / seed_perturb / seed_meas: the simulator's random seeds (rpng_sim's sim_seed_state_init, sim_seed_preturb,
     sim_seed_measurements). runs = K: a Monte-Carlo batch in one process, run r with measurement seed seed_meas + r, on
@@ -40,7 +43,10 @@ def run(exe=None, traj=None, cams=2, clones=11, msckf=10, pts=250, frames=0, cal
     §8). slam_log = PATH writes the per-frame landmark log (--slam-log, single runs). perturb = True starts the filter from a
     calibration perturbed with seed_perturb (seed_perturb + r for run r of a batch; --perturb, needs calib=1); the summary
     gains "perturb" and the RMS of err/σ per calibration block at the first and last frame ("calib_nerr_first",
-    "calib_nerr_last"), with their mean and population standard deviation over a batch."""
+    "calib_nerr_last"), with their mean and population standard deviation over a batch. The estimator options (INTEGRATION.md
+    §8, "Estimator options") are passed as the runner flag of the same name when given (feat_rep_msckf = a representation
+    name; use_fej and the fi_* and calib_* options 0 or 1; the up_* options positive numbers); the summary then lists those
+    that differ from the defaults under "estimator"."""
     cmd = [exe or ENGINE_EXE, "--traj", traj or TRAJ_FIXTURE, "--cams", str(cams), "--clones", str(clones), "--msckf", str(msckf), "--pts", str(pts),
            "--frames", str(frames), "--calib", str(int(calib)), "--integration", integration, "--compress", compress,
            "--seed-init", str(seed_init), "--seed-perturb", str(seed_perturb), "--seed-meas", str(seed_meas)]
@@ -58,6 +64,13 @@ def run(exe=None, traj=None, cams=2, clones=11, msckf=10, pts=250, frames=0, cal
             cmd += [flag, str(v)]
     if perturb:
         cmd += ["--perturb"]
+    estimator = dict(feat_rep_msckf=feat_rep_msckf, use_fej=use_fej, fi_triangulate_1d=fi_triangulate_1d, fi_refine_features=fi_refine_features,
+                     up_msckf_sigma_px=up_msckf_sigma_px, up_msckf_chi2_multipler=up_msckf_chi2_multipler, up_slam_sigma_px=up_slam_sigma_px,
+                     up_slam_chi2_multipler=up_slam_chi2_multipler, calib_cam_extrinsics=calib_cam_extrinsics, calib_cam_intrinsics=calib_cam_intrinsics,
+                     calib_cam_timeoffset=calib_cam_timeoffset, calib_imu_intrinsics=calib_imu_intrinsics, calib_imu_g_sensitivity=calib_imu_g_sensitivity)
+    for name, v in estimator.items():
+        if v is not None:
+            cmd += ["--" + name.replace("_", "-"), str(int(v)) if isinstance(v, bool) else str(v)]
     if capture:
         cmd += ["--capture", str(capture[0]), capture[1]]
     if runs:

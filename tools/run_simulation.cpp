@@ -6,7 +6,10 @@
 //              [--est OUT.txt] [--timing [OUT.csv]] [--capture FRAME PREFIX] [--integration discrete|rk4|analytical]
 //              [--seed-init S] [--seed-perturb S] [--seed-meas S] [--runs K [--jobs J] [--out-dir DIR]] [--consistency [OUT.txt]]
 //              [--cam-model M[,M...]] [--slam M [--slam-in-update U] [--slam-delay S] [--feat-rep-slam NAME] [--slam-log OUT.txt]]
-//              [--perturb]
+//              [--perturb] [--feat-rep-msckf NAME] [--use-fej 0|1] [--fi-triangulate-1d 0|1] [--fi-refine-features 0|1]
+//              [--up-msckf-sigma-px X] [--up-msckf-chi2-multipler X] [--up-slam-sigma-px X] [--up-slam-chi2-multipler X]
+//              [--calib-cam-extrinsics 0|1] [--calib-cam-intrinsics 0|1] [--calib-cam-timeoffset 0|1] [--calib-imu-intrinsics 0|1]
+//              [--calib-imu-g-sensitivity 0|1]
 // Prints one JSON line: frames, ATE (alignment none), mean per-stage host times.
 // --cam-model radtan|equi: the camera model of every camera, or one per camera (a mixed rig, e.g. radtan,equi). Equidistant
 // cameras take the TUM-VI cam0 intrinsics on a 512 x 512 image and the rpng_sim extrinsics of their slot (rpng_sim_cameras
@@ -27,11 +30,18 @@
 // M > 0; so does the JSON line (and every per_run entry), which gains the SLAM and delayed-init status histograms, the mean and
 // maximum live landmarks, the landmarks initialised and marginalised, the anchor changes and the two SLAM stage times.
 // --slam-log OUT.txt (single run, for tests): what every frame did with the landmarks (write_slam_log).
-// --perturb (rpng_sim's sim_do_perturbation; needs --calib 1): the filter starts from a calibration the simulator perturbs
-// with --seed-perturb (Simulator::perturb_parameters), while the measurements and the truth stay the true ones. With
-// --runs, run r also takes perturbation seed seed_perturb + r. The JSON line (and every per_run entry) gains "perturb" and
-// the RMS of err/σ per calibration block at the first and the last frame (calib_nerr_json); a batch, their mean and
-// population standard deviation over the runs.
+// --perturb (rpng_sim's sim_do_perturbation; needs all five calibration blocks on): the filter starts from a calibration the
+// simulator perturbs with --seed-perturb (Simulator::perturb_parameters), while the measurements and the truth stay the true
+// ones. With --runs, run r also takes perturbation seed seed_perturb + r. The JSON line (and every per_run entry) gains
+// "perturb" and the RMS of err/σ per calibration block at the first and the last frame (calib_nerr_json); a batch, their
+// mean and population standard deviation over the runs.
+// Estimator options, named after the keys of the reference's config/rpng_sim/estimator_config.yaml (INTEGRATION.md §8):
+// --feat-rep-msckf NAME (GLOBAL_3D), --use-fej (1), --fi-triangulate-1d (0), --fi-refine-features (1), --up-msckf-sigma-px,
+// --up-msckf-chi2-multipler, --up-slam-sigma-px, --up-slam-chi2-multipler (1 each; the SLAM pair serves the SLAM updates and
+// the delayed initialisation), and one 0|1 flag per calibration block that overrides --calib for that block. A SINGLE MSCKF
+// representation runs as ANCHORED_MSCKF_INVERSE_DEPTH (UpdaterMSCKF.cpp:180-183; the engine remaps it in ovb_api.cu's
+// per-call options, the oracle in msckf_update). The JSON line (and every per_run entry) gains "estimator" with the options
+// that differ from their defaults (estimator_json).
 #ifdef OVB_SIM_ORACLE
 #include "oracle_slam_backend.hpp"
 #elif defined(OVB_SIM_HOST_PROPAGATION)
@@ -62,10 +72,38 @@ struct RunnerOptions {
   int slam = 0, slam_in_update = 25, feat_rep_slam = OVB_REP_GLOBAL_3D;
   double slam_delay = 1.0;
   bool perturb = false;
+  // the estimator options of the flags named after the reference's YAML keys (INTEGRATION.md §8, "Estimator options"):
+  // feat_rep_msckf, do_fej, featinit_options.triangulate_1d / refine_features, msckf_options, slam_options and, once main
+  // has resolved calib_block against --calib, the five do_calib_* flags; every other field stays VioOptions's default
+  VioOptions est;
+  int calib_block[5] = {-1, -1, -1, -1, -1}; // per calib_block_keys entry: 0 / 1 as given, -1 = as --calib
 };
 
 static const char *const rep_names[] = {"GLOBAL_3D", "GLOBAL_FULL_INVERSE_DEPTH", "ANCHORED_3D", "ANCHORED_FULL_INVERSE_DEPTH",
                                         "ANCHORED_MSCKF_INVERSE_DEPTH", "ANCHORED_INVERSE_DEPTH_SINGLE"};
+
+// the calibration blocks of the --calib-* flags (the YAML keys), in RunnerOptions::calib_block's order
+static const char *const calib_block_keys[5] = {"calib_cam_extrinsics", "calib_cam_intrinsics", "calib_cam_timeoffset", "calib_imu_intrinsics",
+                                                "calib_imu_g_sensitivity"};
+static bool *calib_block_flag(VioOptions &v, int b) {
+  bool *const f[5] = {&v.do_calib_camera_pose, &v.do_calib_camera_intrinsics, &v.do_calib_camera_timeoffset, &v.do_calib_imu_intrinsics,
+                      &v.do_calib_imu_g_sensitivity};
+  return f[b];
+}
+// the calib_block_keys index of a --calib-* flag (the key with '-' for '_'), -1 for any other argument
+static int calib_block_of_flag(const std::string &a) {
+  for (int b = 0; b < 5; b++) {
+    std::string flag = std::string("--") + calib_block_keys[b];
+    std::replace(flag.begin(), flag.end(), '_', '-');
+    if (a == flag)
+      return b;
+  }
+  return -1;
+}
+static bool all_calib_blocks(const RunnerOptions &o) {
+  const VioOptions &v = o.est;
+  return v.do_calib_camera_pose && v.do_calib_camera_intrinsics && v.do_calib_camera_timeoffset && v.do_calib_imu_intrinsics && v.do_calib_imu_g_sensitivity;
+}
 
 // a whole decimal integer / number, nothing else
 static bool parse_int(const std::string &a, int &v) {
@@ -81,12 +119,20 @@ static bool parse_double(const std::string &a, double &v) {
   v = std::strtod(a.c_str(), &e);
   return !a.empty() && !*e && std::isfinite(v);
 }
+static bool parse_01(const std::string &a, int &v) { return parse_int(a, v) && (v == 0 || v == 1); }
+static bool parse_rep(const std::string &a, int &v) {
+  const auto it = std::find(std::begin(rep_names), std::end(rep_names), a);
+  v = (int)(it - std::begin(rep_names));
+  return it != std::end(rep_names);
+}
 
 #ifndef OVB_SIM_ORACLE
-// the covariance the engine context must hold: the base state, max_clones + 1 clone poses during the update, max_slam landmarks
-// three wide (one for ANCHORED_INVERSE_DEPTH_SINGLE)
+// the covariance the engine context must hold: the base state (State.cpp:28-131 with the calibration blocks in it), max_clones
+// + 1 clone poses during the update, max_slam landmarks three wide (one for ANCHORED_INVERSE_DEPTH_SINGLE)
 static int state_size_bound(const RunnerOptions &o) {
-  const int base = 15 + (o.calib ? 24 + 1 : 0) + o.cams * (o.calib ? 14 : 0);
+  const VioOptions &v = o.est;
+  const int base = 15 + (v.do_calib_imu_intrinsics ? 15 + (v.do_calib_imu_g_sensitivity ? 9 : 0) : 0) + (v.do_calib_camera_timeoffset ? 1 : 0) +
+                   o.cams * ((v.do_calib_camera_pose ? 6 : 0) + (v.do_calib_camera_intrinsics ? 8 : 0));
   return base + 6 * (o.clones + 1) + o.slam * (o.feat_rep_slam == OVB_REP_ANCHORED_INVERSE_DEPTH_SINGLE ? 1 : 3);
 }
 static const int engine_max_state = 640; // ovb_config::max_state of the runner's engine context
@@ -182,6 +228,40 @@ static std::string calib_nerr_json(const RunnerOptions &o, const RunSummary &s, 
   return ", \"perturb\": true, \"calib_nerr_first\": " + blocks_json(s.nerr_first, fmt) + ", \"calib_nerr_last\": " + blocks_json(s.nerr_last, fmt);
 }
 
+// the estimator options that differ from their defaults (VioOptions's; a calibration block's is --calib's value), as
+// , "estimator": {"use_fej": 0, ...}; empty when none does, so that such a run prints what a run without the flags prints
+static std::string estimator_json(const RunnerOptions &o) {
+  const VioOptions d;
+  VioOptions e = o.est;
+  std::string r;
+  auto add = [&](const char *key, const std::string &v) { r += std::string(r.empty() ? "" : ", ") + "\"" + key + "\": " + v; };
+  auto num = [](double x) {
+    char buf[64];
+    std::snprintf(buf, sizeof(buf), "%.17g", x);
+    return std::string(buf);
+  };
+  if (e.feat_rep_msckf != d.feat_rep_msckf)
+    add("feat_rep_msckf", std::string("\"") + rep_names[e.feat_rep_msckf] + "\"");
+  if (e.do_fej != d.do_fej)
+    add("use_fej", std::to_string((int)e.do_fej));
+  if (e.featinit_options.triangulate_1d != d.featinit_options.triangulate_1d)
+    add("fi_triangulate_1d", std::to_string((int)e.featinit_options.triangulate_1d));
+  if (e.featinit_options.refine_features != d.featinit_options.refine_features)
+    add("fi_refine_features", std::to_string((int)e.featinit_options.refine_features));
+  if (e.msckf_options.sigma_pix != d.msckf_options.sigma_pix)
+    add("up_msckf_sigma_px", num(e.msckf_options.sigma_pix));
+  if (e.msckf_options.chi2_multipler != d.msckf_options.chi2_multipler)
+    add("up_msckf_chi2_multipler", num(e.msckf_options.chi2_multipler));
+  if (e.slam_options.sigma_pix != d.slam_options.sigma_pix)
+    add("up_slam_sigma_px", num(e.slam_options.sigma_pix));
+  if (e.slam_options.chi2_multipler != d.slam_options.chi2_multipler)
+    add("up_slam_chi2_multipler", num(e.slam_options.chi2_multipler));
+  for (int b = 0; b < 5; b++)
+    if (*calib_block_flag(e, b) != (o.calib != 0))
+      add(calib_block_keys[b], std::to_string((int)*calib_block_flag(e, b)));
+  return r.empty() ? "" : ", \"estimator\": {" + r + "}";
+}
+
 static std::string slam_json(const RunnerOptions &o, const RunSummary &s) {
   if (o.slam <= 0)
     return "";
@@ -248,12 +328,10 @@ static RunSummary run_one(const RunnerOptions &o, const std::vector<std::array<d
   sp.seed_preturb = seed_perturb;
   sp.seed_measurements = seed_meas;
   sp.sim_do_perturbation = o.perturb;
-  VioOptions vo;
+  VioOptions vo = o.est;
   vo.num_cameras = o.cams;
   vo.max_clone_size = o.clones;
   vo.max_msckf_in_update = o.msckf;
-  vo.do_calib_camera_pose = vo.do_calib_camera_intrinsics = vo.do_calib_camera_timeoffset = vo.do_calib_imu_intrinsics = vo.do_calib_imu_g_sensitivity =
-      o.calib != 0;
   vo.compress = o.compress == "tsqr" ? OVB_COMPRESS_HOUSEHOLDER_TSQR : (o.compress == "gram" ? OVB_COMPRESS_NORMAL_EQUATIONS : OVB_COMPRESS_CHOLQR2);
   vo.integration_method = o.integration == "discrete" ? INTEGRATION_DISCRETE : (o.integration == "analytical" ? INTEGRATION_ANALYTICAL : INTEGRATION_RK4);
   vo.max_slam_features = o.slam;
@@ -423,7 +501,7 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
       std::snprintf(buf, sizeof(buf), ", \"seed_perturb\": %d", o.seed_perturb + r);
       per_run += buf;
     }
-    per_run += slam_json(o, s) + calib_nerr_json(o, s, "%.17g") + "}";
+    per_run += slam_json(o, s) + calib_nerr_json(o, s, "%.17g") + estimator_json(o) + "}";
   }
   // the same statistics of the per-run mean NEES
   std::string stats;
@@ -458,6 +536,7 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
       stats += ", \"" + key + "_mean\": " + blocks_json(m, "%.17g") + ", \"" + key + "_std\": " + blocks_json(sd, "%.17g");
     }
   }
+  stats += estimator_json(o);
   std::printf("{\"backend\": \"%s\", \"runs\": %d, \"jobs\": %d, \"cams\": %d%s, \"max_clones\": %d, \"max_msckf_in_update\": %d, \"num_pts\": %d, \"calib\": %d, "
               "\"seed_init\": %d, \"seed_perturb\": %d, \"seed_meas\": %d, \"state_dim\": %d, \"map_points\": %zu, \"per_run\": [%s], "
               "\"ate_pos_m_mean\": %.17g, \"ate_pos_m_std\": %.17g, \"ate_ori_deg_mean\": %.17g, \"ate_ori_deg_std\": %.17g, \"frames_total\": %ld, "
@@ -470,7 +549,7 @@ static int run_batch(const RunnerOptions &o, const std::vector<std::array<double
 int main(int argc, char **argv) {
   RunnerOptions o;
   std::string est_path, timing_path, consistency_path, capture_prefix, out_dir, cam_model_arg, slam_log_path;
-  std::string bad_slam; // the first malformed SLAM option
+  std::string bad_slam, bad_est; // the first malformed SLAM / estimator option
   int capture_frame = -1, runs = 0, jobs = 0;
   bool timing = false, consistency = false, cam_model = false;
   for (int i = 1; i < argc; i++) {
@@ -509,14 +588,35 @@ int main(int argc, char **argv) {
     else if (a == "--slam-delay") { const std::string v = next(); if (!parse_double(v, o.slam_delay) || o.slam_delay < 0) bad_slam = a + " " + v; }
     else if (a == "--feat-rep-slam") {
       const std::string v = next();
-      const auto it = std::find(std::begin(rep_names), std::end(rep_names), v);
-      if (it == std::end(rep_names))
+      int rep;
+      if (!parse_rep(v, rep))
         bad_slam = a + " " + v;
       else
-        o.feat_rep_slam = (int)(it - std::begin(rep_names));
+        o.feat_rep_slam = rep;
     }
     else if (a == "--slam-log") slam_log_path = next();
     else if (a == "--perturb") o.perturb = true;
+    else if (a == "--feat-rep-msckf") { const std::string v = next(); if (!parse_rep(v, o.est.feat_rep_msckf)) bad_est = a + " " + v; }
+    else if (a == "--use-fej" || a == "--fi-triangulate-1d" || a == "--fi-refine-features") {
+      const std::string v = next();
+      int x;
+      if (!parse_01(v, x))
+        bad_est = a + " " + v;
+      else
+        (a == "--use-fej" ? o.est.do_fej : a == "--fi-triangulate-1d" ? o.est.featinit_options.triangulate_1d : o.est.featinit_options.refine_features) = x;
+    }
+    else if (a == "--up-msckf-sigma-px" || a == "--up-msckf-chi2-multipler" || a == "--up-slam-sigma-px" || a == "--up-slam-chi2-multipler") {
+      const std::string v = next();
+      UpdaterOptions &u = a.compare(0, 10, "--up-msckf") == 0 ? o.est.msckf_options : o.est.slam_options;
+      double &x = a.find("sigma") != std::string::npos ? u.sigma_pix : u.chi2_multipler;
+      if (!parse_double(v, x) || x <= 0)
+        bad_est = a + " " + v;
+    }
+    else if (const int b = calib_block_of_flag(a); b >= 0) {
+      const std::string v = next();
+      if (!parse_01(v, o.calib_block[b]))
+        bad_est = a + " " + v;
+    }
   }
   if (!bad_slam.empty()) {
     std::fprintf(stderr, "malformed '%s': --slam takes an integer >= 0, --slam-in-update an integer >= 1, --slam-delay seconds >= 0, --feat-rep-slam one of "
@@ -524,8 +624,24 @@ int main(int argc, char **argv) {
                  bad_slam.c_str());
     return 2;
   }
-  if (o.perturb && o.calib == 0) {
-    std::fprintf(stderr, "--perturb needs --calib 1: without online calibration the filter could not estimate the error it starts with\n");
+  if (!bad_est.empty()) {
+    std::fprintf(stderr, "malformed '%s': --feat-rep-msckf takes one of GLOBAL_3D GLOBAL_FULL_INVERSE_DEPTH ANCHORED_3D ANCHORED_FULL_INVERSE_DEPTH "
+                 "ANCHORED_MSCKF_INVERSE_DEPTH ANCHORED_INVERSE_DEPTH_SINGLE, --use-fej, --fi-* and --calib-* 0 or 1, --up-* a number > 0\n",
+                 bad_est.c_str());
+    return 2;
+  }
+  for (int b = 0; b < 5; b++) // a --calib-* flag overrides --calib for its block, wherever either stands
+    *calib_block_flag(o.est, b) = o.calib_block[b] >= 0 ? o.calib_block[b] != 0 : o.calib != 0;
+  if (!o.est.do_calib_imu_intrinsics) { // the state holds Tg only inside the IMU intrinsics (State.h:126-135)
+    if (o.calib_block[4] == 1) {
+      std::fprintf(stderr, "--calib-imu-g-sensitivity 1 needs the IMU intrinsics in the state: Tg is part of them (State.h:126-135)\n");
+      return 2;
+    }
+    o.est.do_calib_imu_g_sensitivity = false;
+  }
+  if (o.perturb && !all_calib_blocks(o)) {
+    std::fprintf(stderr, "--perturb needs all five calibration blocks on (--calib 1 and no --calib-* 0): without online calibration of a block "
+                 "the filter could not estimate the error it starts with\n");
     return 2;
   }
   if (runs > 0 && !slam_log_path.empty()) {
@@ -582,7 +698,7 @@ int main(int argc, char **argv) {
                 "\"mean_ms_propagation\": %.4f, \"mean_ms_msckf_update\": %.4f, \"mean_ms_total\": %.4f, \"map_points\": %zu, \"status_hist\": [%ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld, %ld]%s}\n",
                 backend_name, s.frames, o.cams, cam_model_json(o).c_str(), o.clones, o.msckf, o.pts, o.calib, s.state_dim, s.ate_pos, s.ate_ori_deg, s.feats_in, s.feats_used, s.rows,
                 s.ms_prop, s.ms_msckf, s.ms_total, s.map_points, s.status_hist[0], s.status_hist[1], s.status_hist[2], s.status_hist[3], s.status_hist[4],
-                s.status_hist[5], s.status_hist[6], s.status_hist[7], s.status_hist[8], (nees + slam_json(o, s) + calib_nerr_json(o, s, "%.12g")).c_str());
+                s.status_hist[5], s.status_hist[6], s.status_hist[7], s.status_hist[8], (nees + slam_json(o, s) + calib_nerr_json(o, s, "%.12g") + estimator_json(o)).c_str());
   } catch (const std::exception &e) {
     std::fprintf(stderr, "run_simulation failed: %s\n", e.what());
     return 1;
