@@ -328,6 +328,34 @@ ovb_status ovb_slam_delayed_init_reps(ovb_ctx *ctx, const ovb_frame *frame, cons
                                       const int32_t *feat_rep, const double *sigma_pix, const double *chi2_multipler,
                                       ovb_init_callback on_init, void *user, ovb_feat_out *out, int32_t *lm_off_out);
 
+/* The quaternions behind ovb_frame's rotations (JPL, [x y z w], ov_core/src/types/JPLQuat.h). */
+typedef struct {
+  const double *clone_q; /* [n_clones][4]  PoseJPL::quat() of each clone; clone_R = quat_2_Rot(clone_q) */
+  const double *cam_q;   /* [n_cams][4]    q_ItoC; cam_R = quat_2_Rot(cam_q) */
+} ovb_frame_quat;
+
+/* ovb_slam_delayed_init_reps without the callback: the engine moves its copy of the frame itself between the features,
+ * with the reference's mean update (VioManager::apply_dx): clone and, with do_calib_camera_pose, extrinsic quaternions take
+ * q <- quatnorm([dtheta/2; 1]) (x) q (JPLQuat::update) and R = quat_2_Rot(q); positions and, with
+ * do_calib_camera_intrinsics, intrinsics add their entries of dx. FEJ arrays are never moved (a NULL one follows the value,
+ * as ovb_frame reads it). The arithmetic is include/ovb200_math.hpp's, rounded as the host rounds it, so the features see
+ * the bits a host that applies dx and marshals its frame again would pass.
+ * The caller replays the records in feature order: for every f with lm_off_out[f] >= 0, the new landmark at its triangulated
+ * point (out) moved by dx_new[f] (lm_size entries: 3, or 1 for ANCHORED_INVERSE_DEPTH_SINGLE), then Type::update of every
+ * variable, the new landmark included, with row f of dx (lm_off_out[f] + lm_size entries). P, N, every status and chi2,
+ * lm_off_out, dx_new and dx are bit-identical to ovb_slam_delayed_init_reps with a callback that does that and marshals the
+ * frame again. Rows of features that are not initialised are not written.
+ * Refusals (OVB_ERR_ARG or OVB_ERR_CAPACITY) are those of ovb_slam_delayed_init_reps, plus a NULL quat, dx_new or dx and
+ * an ld_dx below N + the summed landmark widths of the triangulated features. The call can only launch every feature's
+ * work up front when the covariance has room for every triangulated feature: N + that sum above max_state is
+ * OVB_ERR_CAPACITY. On every error P and N are left as they were.
+ * At most two stream synchronisations whatever the number of features: the triangulation's read-back (which feature is initialised
+ * where decides the launches) and the final one of every record. */
+ovb_status ovb_slam_delayed_init_batch(ovb_ctx *ctx, const ovb_frame *frame, const ovb_frame_quat *quat, const ovb_feat_batch *feats,
+                                       const ovb_opts *opts, const int32_t *feat_rep, const double *sigma_pix, const double *chi2_multipler,
+                                       ovb_feat_out *out, int32_t *lm_off_out, double *dx_new /* [n_feats][3] */,
+                                       double *dx /* [n_feats][ld_dx] */, int ld_dx);
+
 /* UpdaterSLAM::perform_anchor_change (update/UpdaterSLAM.cpp:506-647), host math only (no context, no GPU work): re-express an
  * anchored landmark (ovb_opts.feat_rep = one of the ANCHORED_* representations) in a new anchor camera/clone and return
  *   new_value / new_value_fej [3]  the landmark's xyz in the new anchor frame (Landmark::set_from_xyz),
@@ -450,9 +478,9 @@ ovb_status ovb_msckf_shard_finish(ovb_ctx *ctx, double *stacked_dev, int n_block
  * ovb_msckf_shard_compress), counted at the launch, out[1] of which TSQR level kernels,
  * out[2]/out[3] bytes copied host->device / device->host by the last ovb_msckf_update. */
 ovb_status ovb_last_counters(const ovb_ctx *ctx, int64_t out[4]);
-/* The last ovb_slam_delayed_init[_reps] call: out[0] features that reached StateHelper::initialize (triangulated), out[1]
- * stream synchronisations (one for the triangulation, one per such feature), out[2]/out[3] bytes copied host->device /
- * device->host. */
+/* The last ovb_slam_delayed_init[_reps|_batch] call: out[0] features that reached StateHelper::initialize (triangulated), out[1]
+ * stream synchronisations (one for the triangulation, then one per such feature, or one in all for _batch), out[2]/out[3]
+ * bytes copied host->device / device->host. */
 ovb_status ovb_last_init_counters(const ovb_ctx *ctx, int64_t out[4]);
 /* Host wall clock (microseconds) of the last ovb_msckf_update: [0] marshalling into the pinned arena + H2D enqueue,
  * [1] kernel and D2H enqueue, [2] wait for the stream, [3] unpacking the results. */

@@ -27,8 +27,10 @@ UNITS = [
     ("k_ekf.cu", []),
     ("ovb_api.cu", []),
     ("anchor_change.cu", ["-fmad=false"]),  # UpdaterSLAM::perform_anchor_change, one source for the host and the device
+    ("k_init_batch.cu", ["-fmad=false"]),  # the mean update between delayed-init landmarks, include/ovb200_math.hpp's source
 ]
-HEADERS = ["ovb_internal.cuh", "geom.cuh", "chol.cuh", "chol_tiles.cuh", "chi2_table.inc", os.path.join("..", "..", "include", "ovb200.h")]
+HEADERS = ["ovb_internal.cuh", "geom.cuh", "chol.cuh", "chol_tiles.cuh", "chi2_table.inc", os.path.join("..", "..", "include", "ovb200.h"),
+           os.path.join("..", "..", "include", "ovb200_math.hpp")]
 
 
 def _stale(target: str, deps: list[str]) -> bool:

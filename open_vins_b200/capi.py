@@ -98,6 +98,10 @@ class ovb_stats(C.Structure):
                 ("ms_total", C.c_float)]
 
 
+class ovb_frame_quat(C.Structure):
+    _fields_ = [("clone_q", c_double_p), ("cam_q", c_double_p)]
+
+
 INIT_CALLBACK = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int)
 
 
@@ -302,6 +306,8 @@ def load_library(path: str | None = None) -> C.CDLL:
                                          C.POINTER(ovb_feat_out), c_double_p, C.POINTER(ovb_stats)]
     lib.ovb_slam_delayed_init_reps.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts), c_int_p, c_double_p, c_double_p,
                                                INIT_CALLBACK, C.c_void_p, C.POINTER(ovb_feat_out), c_int_p]
+    lib.ovb_slam_delayed_init_batch.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_frame_quat), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts),
+                                                c_int_p, c_double_p, c_double_p, C.POINTER(ovb_feat_out), c_int_p, c_double_p, c_double_p, C.c_int]
     lib.ovb_triangulate.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts),
                                     C.POINTER(ovb_feat_out)]
     lib.ovb_feature_jacobians.argtypes = [vp, C.POINTER(ovb_frame), C.POINTER(ovb_feat_batch), C.POINTER(ovb_opts),
@@ -337,6 +343,7 @@ EXPORTED_SYMBOLS = [
     "ovb_create", "ovb_destroy", "ovb_last_error", "ovb_abi_version", "ovb_opts_default", "ovb_cov_set", "ovb_cov_get",
     "ovb_cov_dim", "ovb_cov_get_marginal", "ovb_cov_clone", "ovb_cov_marginalize", "ovb_cov_propagate", "ovb_cov_propagate_imu", "ovb_cov_initialize",
     "ovb_msckf_update", "ovb_slam_update", "ovb_slam_update_reps", "ovb_set_slam_unbounded", "ovb_slam_delayed_init", "ovb_slam_delayed_init_reps",
+    "ovb_slam_delayed_init_batch",
     "ovb_slam_anchor_change", "ovb_marginalize_window", "ovb_ekf_update", "ovb_triangulate", "ovb_feature_jacobians", "ovb_compress", "ovb_compress_gram", "ovb_compress_cholqr2",
     "ovb_chi2_quantile95", "ovb_last_stage_ms", "ovb_set_replay", "ovb_msckf_replay", "ovb_last_counters", "ovb_last_init_counters", "ovb_last_host_us", "ovb_set_profile", "ovb_profile_read",
     "ovb_set_stream", "ovb_msckf_shard_compress", "ovb_msckf_shard_compress_range", "ovb_shard_partition", "ovb_msckf_shard_finish",
@@ -545,6 +552,30 @@ class Engine:
                                                         _ptr(sp, c_double_p), _ptr(cm, c_double_p), cb, None, C.byref(out.struct()),
                                                         _ptr(lm_off, c_int_p)))
         return out, lm_off
+
+    def slam_delayed_init_batch(self, frame: FrameArrays, clone_q, cam_q, feats: FeatArrays, opts: ovb_opts, sigma_pix=None, chi2_multipler=None,
+                                feat_rep=None):
+        """UpdaterSLAM::delayed_init in one call without a callback: the engine moves its copy of the frame between the
+        features itself, from the JPL quaternions clone_q [n_clones][4] and cam_q [n_cams][4] behind frame.clone_R / cam_R.
+        Returns (FeatOut, lm_off, dx_new [F][3], dx [F][N + 3F]); the caller replays them in feature order: for every f with
+        lm_off[f] >= 0, the landmark at its triangulated point moved by dx_new[f][:lm_size], then every variable moved by
+        dx[f][:lm_off[f] + lm_size]. Rows of features that were not initialised stay NaN."""
+        F = feats.n_feats
+        out = FeatOut(F)
+        lm_off = np.full(F, -1, dtype=np.int32)
+        ld = self.cov_dim() + 3 * F
+        dx_new = np.full((F, 3), np.nan)
+        dx = np.full((F, max(ld, 1)), np.nan)
+        cq = np.ascontiguousarray(clone_q, dtype=np.float64).reshape(frame.n_clones, 4)
+        kq = np.ascontiguousarray(cam_q, dtype=np.float64).reshape(frame.n_cams, 4)
+        quat = ovb_frame_quat(_ptr(cq, c_double_p), _ptr(kq, c_double_p))
+        sp = None if sigma_pix is None else np.ascontiguousarray(sigma_pix, dtype=np.float64)
+        cm = None if chi2_multipler is None else np.ascontiguousarray(chi2_multipler, dtype=np.float64)
+        reps = None if feat_rep is None else np.ascontiguousarray(feat_rep, dtype=np.int32)
+        self._check(self.lib.ovb_slam_delayed_init_batch(self.h, C.byref(frame.struct()), C.byref(quat), C.byref(feats.struct()), C.byref(opts),
+                                                         _ptr(reps, c_int_p), _ptr(sp, c_double_p), _ptr(cm, c_double_p), C.byref(out.struct()),
+                                                         _ptr(lm_off, c_int_p), _ptr(dx_new, c_double_p), _ptr(dx, c_double_p), int(dx.shape[1])))
+        return out, lm_off, dx_new, dx
 
     def triangulate(self, frame: FrameArrays, feats: FeatArrays, opts: ovb_opts):
         out = FeatOut(feats.n_feats)

@@ -489,14 +489,17 @@ void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bo
 //   M = Hx P[cols, cols] Hx' + s2 I (k x k, upper triangle mirrored like selfadjointView<Upper>)
 //   P[0:N, N:N+k] = -m Hinv',  P[N:N+k, 0:N] = its transpose,  P[N:N+k, N:N+k] = Hinv M Hinv'
 // Single CTA (N <= a few hundred rows, k <= 3): the step is a serial point in the reference as well.
-__global__ void k_cov_init_augment(double *__restrict__ P, int ld, int N, int k, int n, const DevUpdateInfo *__restrict__ info,
-                                   const double *__restrict__ Hx, const double *__restrict__ Hinv, double sigma2, const int *__restrict__ skip) {
+// N_dev (optional): N is read there (ovb_slam_delayed_init_batch: the size the gates before have left); N_max sizes m
+__global__ void k_cov_init_augment(double *__restrict__ P, int ld, int N_max, int k, int n, const DevUpdateInfo *__restrict__ info,
+                                   const double *__restrict__ Hx, const double *__restrict__ Hinv, double sigma2, const int *__restrict__ skip,
+                                   const int *__restrict__ N_dev) {
   extern __shared__ double ism[]; // m[N][k], then M[k][k]
-  double *m = ism, *M = ism + (size_t)N * k;
+  double *m = ism, *M = ism + (size_t)N_max * k;
   OVB_PDL_ENTER();
   const int tid = threadIdx.x;
   if (skip && *skip)
     return;
+  const int N = N_dev ? *N_dev : N_max;
   for (int a = tid; a < N; a += blockDim.x) {
     for (int i = 0; i < k; i++) {
       double acc = 0.0;
@@ -544,7 +547,8 @@ __global__ void k_cov_init_augment(double *__restrict__ P, int ld, int N, int k,
   }
 }
 
-bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, const double *Hinv_dev, double sigma2, const int *skip_dev) {
+bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, const double *Hinv_dev, double sigma2, const int *skip_dev,
+                             const int *N_dev) {
   const int N = ctx->N;
   size_t smem = sizeof(double) * ((size_t)N * k + (size_t)k * k);
   if (smem > 200 * 1024)
@@ -554,7 +558,7 @@ bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, c
     ctx->attr_done[5] = 1;
   }
   return ovb_launch(ctx, k_cov_init_augment, dim3(1), dim3(256), smem, ctx->P[ctx->cur], ctx->ldP, N, k, n, ctx->d_info, Hx_dev, Hinv_dev, sigma2,
-                    skip_dev) == cudaSuccess;
+                    skip_dev, N_dev) == cudaSuccess;
 }
 
 // ovb_slam_delayed_init, after the per-feature kernel: the head of the init system (status, chi2, skip flag), H_L^-1 of the

@@ -117,6 +117,25 @@ struct DevInitSys {
 };
 #define OVB_INIT_HEAD_BYTES (4 * sizeof(int) + 4 * sizeof(double))
 
+// ovb_slam_delayed_init_batch: what the device needs to move the frame between the features and what it hands back.
+// One allocation [DevInitBatch][DevInitRec x F][dx rows]; the head is uploaded once, everything is read back once.
+struct DevInitBatch {
+  int N;                                // live covariance size: advances by a landmark's width when it is initialised
+  int fej_R_is_value, fej_p_is_value;   // the caller passed no FEJ array: the FEJ copy follows the moved value
+  int pad;
+  double clone_q[OVB_MAX_CLONES][4];    // JPL [x y z w] behind DevFrame::clone_R
+  double cam_q[OVB_MAX_CAMS][4];        // behind DevFrame::cam_R
+};
+struct DevInitRec {
+  int status;          // after the gate; OVB_FEAT_OK = initialised
+  int lm_off;          // the landmark's covariance id, -1 when it was not initialised
+  int fail;            // 0, or what makes the call fail at this feature: 1 H_L rank deficient, 2 column count, 3 EKF update
+  int n;               // columns the per-feature kernel counted (fail 2)
+  int not_spd, nonfinite, neg_diag_index, pad; // the EKF update's flags (fail 3)
+  double chi2;
+  double dx_new[3];
+};
+
 // ovb_marginalize_window: the frame slice the anchor changes read (FEJ arrays already substituted when the caller has
 // none) and one record per re-anchored landmark; uploaded with the rest of the call's inputs in one H2D copy
 struct DevWinFrame {
@@ -250,6 +269,9 @@ struct ovb_ctx {
   // the counters of the last call (ovb_last_init_counters)
   DevInitSys *d_init, *h_init;
   int64_t init_counters[4];
+  // ovb_slam_delayed_init_batch: [DevInitBatch][DevInitRec x F][dx rows] on the device and its pinned mirror (grown on demand)
+  unsigned char *d_ib, *h_ib;
+  size_t ib_cap; // bytes
   // ovb_cov_propagate_imu: the per-step operands [F | G | qc | dnc_dt | old indices], one H2D copy per call; the pinned
   // side also receives Phi and Q. Reserved at ovb_create for ordinary frames, grown with headroom beyond.
   double *d_imu, *h_imu;
@@ -317,8 +339,13 @@ void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bo
                        const int *skip_dev = nullptr);
 // false: the launch was refused (shared-memory footprint) or failed; the caller must not grow N.
 // skip_dev (optional): the kernel returns without writing when *skip_dev is nonzero
+// N_dev (optional): the covariance size is read on the device (ctx->N is then its upper bound and sizes the launch)
 bool launch_cov_init_augment(ovb_ctx *ctx, int k, int n, const double *Hx_dev, const double *Hinv_dev, double sigma2,
-                             const int *skip_dev = nullptr);
+                             const int *skip_dev = nullptr, const int *N_dev = nullptr);
+// ovb_slam_delayed_init_batch, after feature `feat`'s EKF update: its record (the dx row, N0 + k doubles, at dx_row), and
+// unless the feature was skipped or failed, the StateHelper::EKFUpdate mean update (⊞) of the device frame with d_dx and
+// the advance of the live covariance size by k. Compiled without FMA contraction: the frame gets the host's bits.
+void launch_init_commit(ovb_ctx *ctx, DevInitBatch *ib, DevInitRec *rec, double *dx_row, int k, int calib_pose, int calib_intr);
 // neg_diag_dev (optional): d_info's negative-diagonal flag of a propagation enqueued before; when it is set the clone
 // leaves P alone (ovb_cov_propagate_imu then does not grow N)
 void launch_cov_clone(ovb_ctx *ctx, int old_off, int size, const double *dnc_dt_dev, int dt_off, const int *neg_diag_dev = nullptr);
