@@ -35,6 +35,16 @@ __device__ __forceinline__ void ct_dmma2k8(double &d0, double &d1, double &e0, d
                : "+d"(d0), "+d"(d1), "+d"(e0), "+d"(e1)
                : "d"(a00), "d"(a10), "d"(a01), "d"(a11), "d"(b0), "d"(b1));
 }
+// [D0; D1] += [A0; A1] B with k = 0..15, m16n8k16: a[i] = A[g + 8(i&1)][q + 4(i>>1)] (A = [A0; A1], 16 x 16),
+// b[j] = B[q + 4j][g]. Same bits as four chained ct_dmma2 over k 0-3, 4-7, 8-11, 12-15, and as the sixteen chained
+// fma(a_k, b_k, d) of each output in ascending k (tools/ubench/fp64_rate.cu checks both), in less pipe time.
+__device__ __forceinline__ void ct_dmma2k16(double &d0, double &d1, double &e0, double &e1, const double (&a)[8], const double (&b)[4]) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, "
+               "{%0,%1,%2,%3};"
+               : "+d"(d0), "+d"(d1), "+d"(e0), "+d"(e1)
+               : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]), "d"(b[2]),
+                 "d"(b[3]));
+}
 __device__ __forceinline__ int ct_tri(int b) { return (b * (b + 1)) >> 1; }
 __device__ __forceinline__ void ct_bar_group(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 // element (i, j), j <= i, of a tile-packed triangle

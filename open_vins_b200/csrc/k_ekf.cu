@@ -7,7 +7,7 @@
 //                            P <- sym_U(P - Y Y')      dx = Y w
 // (K M' = M S^-1 M' = Y Y' and K res = Y w, so neither S^-1 nor K is formed; the reference forms both.)
 // P is row-major with a fixed leading dimension so clone() grows it in place.
-#include "chol.cuh"
+#include "chol_tiles.cuh"
 #include "ovb_internal.cuh"
 
 #define EK_T 32
@@ -253,149 +253,186 @@ __global__ void __launch_bounds__(256) k_ekf_downdate(double *__restrict__ P, in
 
 // ---- one-shot variants for K <= EK1_KMAX (the whole inner dimension staged at once: a CTA pays ONE L2 round trip instead
 // of one per 32-wide K tile; at config-2 sizes these products are latency-, not flop-bound). Same contract as k_ekf_gemm.
+// Each CTA computes a 16 x 8 output tile on the FP64 tensor cores, m16n8k16 per 16 k (ct_dmma2k16): each output is the
+// chain acc = fma(a_k, b_k, acc) over ascending k from zero, the bits of the scalar loops before (the instruction gives the
+// chained DFMA's bits, tools/ubench/fp64_rate.cu). K is padded to a multiple of 16 with zeros, which leave a chain that
+// starts at +0 unchanged. Small tiles give the grid enough CTAs to cover the SMs (config 2: 260, 110, 169). The DMMA chain
+// is one warp's; the CTA's four warps share the issue of the staging copies, which one warp alone spends longer on.
 #define EK1_KMAX 160
+#define EK1_M 16 // output rows per CTA
+#define EK1_N 8  // output columns per CTA
+#define EK1_T 128
 __device__ __forceinline__ void ek_cpa8(double *dst_smem, const double *src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((unsigned)__cvta_generic_to_shared(dst_smem)), "l"(src) : "memory");
 }
-__global__ void __launch_bounds__(256) k_ekf_gemm1(int mode, const double *__restrict__ P, int ldP, const double *__restrict__ H, int ldH,
-                                                   const double *__restrict__ Min, int ldM, const DevUpdateInfo *__restrict__ info, int X, int Y,
-                                                   int K, double *__restrict__ Cout, int ldC, double sigma2, const double *__restrict__ Rdiag) {
-  OVB_PDL_ENTER();
-  extern __shared__ __align__(16) double g1[];
-  const int x0 = blockIdx.x * EK_T, y0 = blockIdx.y * EK_T;
-  if (mode == 1 && y0 > x0 + EK_T - 1)
-    return; // strictly upper tile of S
-  const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
-  const int *cs = info->col_state;
-  const int pk = K | 1;
-  // mode 0: Gs[j][a] = P[cs[j]][x0+a] (K x 32, pitch 33)   Hs[i][j] = H[y0+i][j] (32 x K, pitch pk)      M[a][i]
-  // mode 1: Hs[i][j] = H[x0+i][j]      (32 x K, pitch pk)   Gs[j][k] = M[cs[j]][y0+k] (K x 32, pitch 33)   S[i][k]
-  double *Gs = g1, *Hs = g1 + (size_t)K * 33;
-  const double *Gsrc = (mode == 0) ? P : Min;
-  const int ldG = (mode == 0) ? ldP : ldM;
-  const int g0 = (mode == 0) ? x0 : y0, gmax = (mode == 0) ? X : Y;
-  const int h0 = (mode == 0) ? y0 : x0, hmax = (mode == 0) ? Y : X;
-  // the column map first (the gathered rows' addresses depend on it), then every element of both operands as an 8-byte
-  // cp.async: one L2 round trip for the whole staging instead of a dependent index -> element pair per loop trip
-  __shared__ int cs_s[EK1_KMAX];
-  for (int j = tid; j < K; j += 256)
-    cs_s[j] = cs[j];
-  __syncthreads();
-  for (int e = tid; e < K * 32; e += 256) {
-    const int j = e >> 5, a = e & 31;
-    if (g0 + a < gmax)
-      ek_cpa8(&Gs[j * 33 + a], &Gsrc[(size_t)cs_s[j] * ldG + g0 + a]);
-    else
-      Gs[j * 33 + a] = 0.0;
-  }
-  for (int i = ty; i < 32; i += 8)
-    for (int j = tx; j < K; j += 32) {
-      if (h0 + i < hmax)
-        ek_cpa8(&Hs[i * pk + j], &H[(size_t)(h0 + i) * ldH + j]);
+__host__ __device__ __forceinline__ int ek1_kpad(int K) { return (K + 15) & ~15; }
+// An operand of R rows (A: 16, B: 8) over Kp = ek1_kpad(K) k, staged in one of two layouts, both read without bank conflicts
+// by the fragment loads:  row-major  X[x][k] at x (Kp + 4) + k  (source rows contiguous in k; warp w copies rows w, w+4, ..)
+//                         k-major    X[x][k] at k (R + 4) + x   (source columns contiguous in x: the rows gathered by cs)
+// Outside [0, xmax) x [0, K) the operand is zero.
+template <int R> __device__ __forceinline__ void ek1_stage_rows(double *dst, int Kp, const double *src, size_t ld, int x0, int xmax, int K) {
+  const int lane = threadIdx.x & 31;
+  for (int x = threadIdx.x >> 5; x < R; x += EK1_T / 32)
+    for (int k = lane; k < Kp; k += 32) {
+      if (x0 + x < xmax && k < K)
+        ek_cpa8(&dst[x * (Kp + 4) + k], &src[(size_t)(x0 + x) * ld + k]);
       else
-        Hs[i * pk + j] = 0.0;
+        dst[x * (Kp + 4) + k] = 0.0;
     }
+}
+template <int R> __device__ __forceinline__ void ek1_stage_cols(double *dst, int Kp, const double *src, size_t ld, const int *cs_s, int x0, int xmax, int K) {
+  const int x = threadIdx.x % R;
+  for (int k = threadIdx.x / R; k < Kp; k += EK1_T / R) {
+    if (x0 + x < xmax && k < K)
+      ek_cpa8(&dst[k * (R + 4) + x], &src[(size_t)cs_s[k] * ld + x0 + x]);
+    else
+      dst[k * (R + 4) + x] = 0.0;
+  }
+}
+__device__ __forceinline__ void ek1_stage_wait() {
   asm volatile("cp.async.commit_group;" ::: "memory");
   asm volatile("cp.async.wait_group 0;" ::: "memory");
   __syncthreads();
-  double acc[4] = {0, 0, 0, 0};
-  if (mode == 0) {
-    // acc[u] = sum_j Gs[j][tx] * Hs[ty + 8u][j]   -> M[x0 + tx][y0 + ty + 8u]
-    for (int j = 0; j < K; j++) {
-      const double gv = Gs[j * 33 + tx];
+}
+// c = A B over k < Kp for the warp's 16 x 8 tile; A_KMAJOR / B_KMAJOR: the operands' layouts. Lane (g, q) = (lane>>2,
+// lane&3) ends with c[0], c[1] = C[g][2q], C[g][2q+1] and c[2], c[3] = C[g+8][2q], C[g+8][2q+1].
+template <bool A_KMAJOR, bool B_KMAJOR> __device__ __forceinline__ void ek1_mma_tile(const double *As, const double *Bs, int Kp, double (&c)[4]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  const int asx = A_KMAJOR ? 1 : Kp + 4, ask = A_KMAJOR ? EK1_M + 4 : 1;
+  const int bsx = B_KMAJOR ? 1 : Kp + 4, bsk = B_KMAJOR ? EK1_N + 4 : 1;
+  const double *ap = As + g * asx + q * ask, *bp = Bs + g * bsx + q * bsk;
+  c[0] = c[1] = c[2] = c[3] = 0.0;
+#pragma unroll 2
+  for (int kb = 0; kb < Kp; kb += 16) {
+    double a[8], b[4];
 #pragma unroll
-      for (int u = 0; u < 4; u++)
-        acc[u] += gv * Hs[(ty + 8 * u) * pk + j];
-    }
+    for (int i = 0; i < 8; i++)
+      a[i] = ap[8 * (i & 1) * asx + (kb + 4 * (i >> 1)) * ask];
 #pragma unroll
-    for (int u = 0; u < 4; u++) {
-      const int a = x0 + tx, i = y0 + ty + 8 * u;
-      if (a < X && i < Y)
-        Cout[(size_t)a * ldC + i] = acc[u];
-    }
-  } else {
-    // acc[u] = sum_j Hs[ty + 8u][j] * Gs[j][tx]   -> S[x0 + ty + 8u][y0 + tx]
-    for (int j = 0; j < K; j++) {
-      const double gv = Gs[j * 33 + tx];
+    for (int j = 0; j < 4; j++)
+      b[j] = bp[(kb + 4 * j) * bsk];
+    ct_dmma2k16(c[0], c[1], c[2], c[3], a, b);
+  }
+}
+
+__global__ void __launch_bounds__(EK1_T) k_ekf_gemm1(int mode, const double *__restrict__ P, int ldP, const double *__restrict__ H, int ldH,
+                                                     const double *__restrict__ Min, int ldM, const DevUpdateInfo *__restrict__ info, int X, int Y,
+                                                     int K, double *__restrict__ Cout, int ldC, double sigma2, const double *__restrict__ Rdiag) {
+  // Programmatic dependent launch, in the order that lets mode 1 read H and the column map before its wait: mode 0 waits
+  // BEFORE it lets its dependant (mode 1) launch, so when mode 1 runs, k_ekf_prep and every kernel before it (k_cq_trmm,
+  // which writes H; k_init_prep, which writes the column map on the landmark-initialisation paths) have completed. Only M,
+  // mode 0's output, is read after mode 1's wait. Mode 0 itself reads nothing before its wait.
+  if (mode == 0)
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  extern __shared__ __align__(16) double g1[];
+  __shared__ int cs_s[EK1_KMAX];
+  const int x0 = blockIdx.x * EK1_M, y0 = blockIdx.y * EK1_N;
+  if (mode == 1 && y0 > x0 + EK1_M - 1)
+    return; // strictly upper tile of S
+  const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, q = lane & 3;
+  const int Kp = ek1_kpad(K);
+  // A: Kp x 20 doubles (either layout fits), then B: Kp x 12
+  double *As = g1, *Bs = g1 + (size_t)Kp * (EK1_M + 4);
+  // H's rows first: their copies are in flight while the column map, which the gathered operand's addresses need, arrives
+  // (mode 1: both before the wait)
+  if (mode == 0)
+    ek1_stage_rows<EK1_N>(Bs, Kp, H, (size_t)ldH, y0, Y, K);
+  else
+    ek1_stage_rows<EK1_M>(As, Kp, H, (size_t)ldH, x0, X, K);
+  const int *cs = info->col_state;
+  for (int j = tid; j < K; j += EK1_T)
+    cs_s[j] = cs[j];
+  if (mode == 1)
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+  __syncthreads();
+  // M[a][i] = sum_j P[cs[j]][a] H[i][j]: A = P's gathered rows (k-major), B = H's rows (row-major)
+  // S[i][k] = sum_j H[i][j] M[cs[j]][k]: A = H's rows (row-major), B = M's gathered rows (k-major)
+  if (mode == 0)
+    ek1_stage_cols<EK1_M>(As, Kp, P, (size_t)ldP, cs_s, x0, X, K);
+  else
+    ek1_stage_cols<EK1_N>(Bs, Kp, Min, (size_t)ldM, cs_s, y0, Y, K);
+  ek1_stage_wait();
+  if (tid >= 32)
+    return;
+  double c[4];
+  if (mode == 0)
+    ek1_mma_tile<true, false>(As, Bs, Kp, c);
+  else
+    ek1_mma_tile<false, true>(As, Bs, Kp, c);
 #pragma unroll
-      for (int u = 0; u < 4; u++)
-        acc[u] += Hs[(ty + 8 * u) * pk + j] * gv;
-    }
-#pragma unroll
-    for (int u = 0; u < 4; u++) {
-      const int i = x0 + ty + 8 * u, k = y0 + tx;
-      if (i < X && k < Y) {
-        double v = acc[u];
-        if (i == k)
-          v += Rdiag ? Rdiag[i] : sigma2;
-        Cout[(size_t)i * ldC + k] = v;
-      }
+  for (int u = 0; u < 4; u++) {
+    const int x = x0 + g + 8 * (u >> 1), y = y0 + 2 * q + (u & 1);
+    if (x < X && y < Y) {
+      double v = c[u];
+      if (mode == 1 && x == y)
+        v += Rdiag ? Rdiag[x] : sigma2;
+      Cout[(size_t)x * ldC + y] = v;
     }
   }
 }
 
-// P <- sym_U(P - Y Y'), dx = Y w, r <= EK1_KMAX: both 32-row strips of Y staged at once (same contract as k_ekf_downdate)
-__global__ void __launch_bounds__(256) k_ekf_downdate1(double *__restrict__ P, int ldP, const double *__restrict__ Yin, int ldY, int N, int r,
-                                                       const double *__restrict__ w, double *__restrict__ dx, DevUpdateInfo *__restrict__ info) {
+// P <- sym_U(P - Y Y'), dx = Y w, r <= EK1_KMAX (same contract as k_ekf_downdate): the 16 x 8 tile of P at rows a0.., columns
+// b0.. from rows a0.. and b0.. of Y; tiles wholly below the diagonal exit. Warp 0 runs the DMMA chain and writes P; on the
+// tile with b0 == a0, warp 1 computes dx[a0..a0+16) beside it. Smem: Y's rows a0.. (16 x (Kp + 4)), rows b0..
+// (8 x (Kp + 4)), then w (r).
+__global__ void __launch_bounds__(EK1_T, 1) k_ekf_downdate1(double *__restrict__ P, int ldP, const double *__restrict__ Yin, int ldY, int N, int r,
+                                                         const double *__restrict__ w, double *__restrict__ dx, DevUpdateInfo *__restrict__ info) {
   OVB_PDL_ENTER();
   extern __shared__ __align__(16) double d1[];
-  const int a0 = blockIdx.x * EK_T, b0 = blockIdx.y * EK_T;
-  if (b0 < a0)
+  const int a0 = blockIdx.x * EK1_M, b0 = blockIdx.y * EK1_N;
+  if (b0 + EK1_N - 1 < a0)
     return;
-  const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
-  if (info->not_spd) { // failed factor: P stays as it was, no correction
-    if (a0 == b0 && tid < EK_T && a0 + tid < N)
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, g = lane >> 2, q = lane & 3;
+  const bool dx_tile = b0 == a0;
+  const int Kp = ek1_kpad(r);
+  double *As = d1, *Bs = As + (size_t)EK1_M * (Kp + 4), *ws = Bs + (size_t)EK1_N * (Kp + 4);
+  // the copies, warp 0's entries of P and the factor's verdict all in flight at once (Y is staged before the verdict is
+  // known, and used only when the factor succeeded)
+  ek1_stage_rows<EK1_M>(As, Kp, Yin, (size_t)ldY, a0, N, r);
+  ek1_stage_rows<EK1_N>(Bs, Kp, Yin, (size_t)ldY, b0, N, r);
+  if (dx_tile)
+    for (int k = tid; k < r; k += EK1_T)
+      ek_cpa8(&ws[k], &w[k]);
+  double pv[4];
+#pragma unroll
+  for (int u = 0; u < 4; u++) {
+    const int a = a0 + g + 8 * (u >> 1), b = b0 + 2 * q + (u & 1);
+    pv[u] = (wid == 0 && a < N && b < N && b >= a) ? P[(size_t)a * ldP + b] : 0.0;
+  }
+  const int not_spd = info->not_spd;
+  ek1_stage_wait();
+  if (not_spd) { // failed factor: P stays as it was, no correction
+    if (dx_tile && tid < EK1_M && a0 + tid < N)
       dx[a0 + tid] = 0.0;
     return;
   }
-  const int pk = r | 1;
-  double *As = d1, *Bs = d1 + (size_t)32 * pk, *ws = Bs + (size_t)32 * pk;
-  for (int i = ty; i < 32; i += 8)
-    for (int k = tx; k < r; k += 32) {
-      if (a0 + i < N)
-        ek_cpa8(&As[i * pk + k], &Yin[(size_t)(a0 + i) * ldY + k]);
-      else
-        As[i * pk + k] = 0.0;
-      if (b0 + i < N)
-        ek_cpa8(&Bs[i * pk + k], &Yin[(size_t)(b0 + i) * ldY + k]);
-      else
-        Bs[i * pk + k] = 0.0;
-    }
-  for (int k = tid; k < r; k += 256)
-    ek_cpa8(&ws[k], &w[k]);
-  asm volatile("cp.async.commit_group;" ::: "memory");
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
-  __syncthreads();
-  double acc[4] = {0, 0, 0, 0};
-  for (int k = 0; k < r; k++) {
-    const double bv = Bs[tx * pk + k];
+  if (wid == 0) {
+    double c[4];
+    ek1_mma_tile<false, false>(As, Bs, Kp, c);
 #pragma unroll
-    for (int u = 0; u < 4; u++)
-      acc[u] += As[(ty + 8 * u) * pk + k] * bv;
-  }
-#pragma unroll
-  for (int u = 0; u < 4; u++) {
-    const int a = a0 + ty + 8 * u, b = b0 + tx;
-    if (a < N && b < N && b >= a) {
-      const double v = P[(size_t)a * ldP + b] - acc[u];
-      P[(size_t)a * ldP + b] = v;
-      P[(size_t)b * ldP + a] = v;
-      if (a == b && v < 0.0)
-        atomicMin(&info->neg_diag_index, a);
-      if (!isfinite(v))
-        info->nonfinite = 1;
+    for (int u = 0; u < 4; u++) {
+      const int a = a0 + g + 8 * (u >> 1), b = b0 + 2 * q + (u & 1);
+      if (a < N && b < N && b >= a) {
+        const double v = pv[u] - c[u];
+        P[(size_t)a * ldP + b] = v;
+        P[(size_t)b * ldP + a] = v;
+        if (a == b && v < 0.0)
+          atomicMin(&info->neg_diag_index, a);
+        if (!isfinite(v))
+          info->nonfinite = 1;
+      }
     }
-  }
-  if (a0 == b0 && tid < EK_T && a0 + tid < N) {
-    double s0 = 0.0, s1 = 0.0;
-    int k = 0;
-    for (; k + 1 < r; k += 2) {
-      s0 += As[tid * pk + k] * ws[k];
-      s1 += As[tid * pk + k + 1] * ws[k + 1];
-    }
-    if (k < r)
-      s0 += As[tid * pk + k] * ws[k];
-    dx[a0 + tid] = s0 + s1;
+  } else if (wid == 1 && dx_tile) {
+    // dx[a] = s0 + s1, s0 over the even k and s1 over the odd k (ascending): lanes 0-15 carry s0 of rows a0 + lane, lanes
+    // 16-31 s1 of the same rows
+    const double *Ar = As + (lane & 15) * (Kp + 4);
+    double s = 0.0;
+    for (int k = lane >> 4; k < r; k += 2)
+      s = fma(Ar[k], ws[k], s);
+    const double s1 = __shfl_down_sync(0xffffffffu, s, 16);
+    if (lane < EK1_M && a0 + lane < N)
+      dx[a0 + lane] = s + s1;
   }
 }
 
@@ -433,13 +470,14 @@ void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bo
   }
   // small inner dimensions (config 2: n = r = 154): one-shot staged products, DMMA Cholesky + register solve of k_cholqr.cu
   const bool one_shot = ctx->ekf_chol_dmma && n <= EK1_KMAX && r <= EK1_KMAX;
-  dim3 g0((N + EK_T - 1) / EK_T, (r + EK_T - 1) / EK_T);
-  dim3 g1((r + EK_T - 1) / EK_T, (r + EK_T - 1) / EK_T);
   if (one_shot) {
-    const size_t sm01 = sizeof(double) * ((size_t)n * 33 + (size_t)32 * (n | 1));
-    ovb_launch(ctx, k_ekf_gemm1, dim3(g0), dim3(256), sm01, 0, P, ld, H, ldHm, nullptr, 0, ctx->d_info, N, r, n, ctx->d_M, ld, 0.0, nullptr);
-    ovb_launch(ctx, k_ekf_gemm1, dim3(g1), dim3(256), sm01, 1, P, ld, H, ldHm, ctx->d_M, ld, ctx->d_info, r, r, n, ctx->d_S, ld, sigma2, Rdiag_dev);
+    const size_t sm01 = sizeof(double) * (size_t)ek1_kpad(n) * (EK1_M + 4 + EK1_N + 4);
+    const dim3 t0((N + EK1_M - 1) / EK1_M, (r + EK1_N - 1) / EK1_N), t1((r + EK1_M - 1) / EK1_M, (r + EK1_N - 1) / EK1_N);
+    ovb_launch(ctx, k_ekf_gemm1, t0, dim3(EK1_T), sm01, 0, P, ld, H, ldHm, nullptr, 0, ctx->d_info, N, r, n, ctx->d_M, ld, 0.0, nullptr);
+    ovb_launch(ctx, k_ekf_gemm1, t1, dim3(EK1_T), sm01, 1, P, ld, H, ldHm, ctx->d_M, ld, ctx->d_info, r, r, n, ctx->d_S, ld, sigma2, Rdiag_dev);
   } else {
+    dim3 g0((N + EK_T - 1) / EK_T, (r + EK_T - 1) / EK_T);
+    dim3 g1((r + EK_T - 1) / EK_T, (r + EK_T - 1) / EK_T);
     ovb_launch(ctx, k_ekf_gemm, dim3(g0), dim3(256), (size_t)(0), 0, P, ld, H, ldHm, nullptr, 0, ctx->d_info, N, r, n, ctx->d_M, ld, 0.0, nullptr);
     ovb_launch(ctx, k_ekf_gemm, dim3(g1), dim3(256), (size_t)(0), 1, P, ld, H, ldHm, ctx->d_M, ld, ctx->d_info, r, r, n, ctx->d_S, ld, sigma2, Rdiag_dev);
   }
@@ -472,11 +510,12 @@ void launch_ekf_update(ovb_ctx *ctx, const double *H, int ldHm, int r, int n, bo
     ovb_launch(ctx, k_ekf_trsm, dim3((N + TR_ROWS - 1) / TR_ROWS), dim3(32 * TR_ROWS), (size_t)(L_in_smem ? trsm_full : trsm_small), ctx->d_M, ld, ctx->d_S, ld, invdiag, N,
                r, ctx->d_Y, ld, L_in_smem, ctx->d_info);
   }
-  dim3 g2((N + EK_T - 1) / EK_T, (N + EK_T - 1) / EK_T);
   if (one_shot) {
-    const size_t smd = sizeof(double) * ((size_t)64 * (r | 1) + r);
-    ovb_launch(ctx, k_ekf_downdate1, dim3(g2), dim3(256), smd, P, ld, Yd, ld, N, r, ctx->d_w, ctx->d_dx, ctx->d_info);
+    const size_t smd = sizeof(double) * ((size_t)(EK1_M + EK1_N) * (ek1_kpad(r) + 4) + r);
+    const dim3 t2((N + EK1_M - 1) / EK1_M, (N + EK1_N - 1) / EK1_N);
+    ovb_launch(ctx, k_ekf_downdate1, t2, dim3(EK1_T), smd, P, ld, Yd, ld, N, r, ctx->d_w, ctx->d_dx, ctx->d_info);
   } else {
+    dim3 g2((N + EK_T - 1) / EK_T, (N + EK_T - 1) / EK_T);
     ovb_launch(ctx, k_ekf_downdate, dim3(g2), dim3(256), (size_t)(0), P, ld, Yd, ld, N, r, ctx->d_w, ctx->d_dx, ctx->d_info);
   }
 }

@@ -3,7 +3,9 @@
 //   * throughput per SM at 1-16 warps per SM (one CTA per SM, 8 independent accumulators per warp)
 //   * dependent-issue latency of each shape (one warp, one accumulator chain)
 //   * bit identity on random inputs, with and without cancellation: one m16n8k4 against its two m8n8k4 halves, one
-//     m16n8k8 against two chained m16n8k4 (k 0-3, then 4-7), one m16n8k16 against four chained m16n8k4
+//     m16n8k8 against two chained m16n8k4 (k 0-3, then 4-7), one m16n8k16 against four chained m16n8k4; and the tensor
+//     core against scalar DFMA: m8n8k4 and m16n8k4 against four chained fma.rn.f64 in ascending k starting from C, four
+//     chained m16n8k4 against sixteen
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_rate fp64_rate.cu
 #include <cmath>
 #include <cstdio>
@@ -97,10 +99,12 @@ template <class S> __global__ void k_mma_chain(double *out, int iters, long long
 //   way 0  k 0-3 : two m8n8k4 (rows 0-7, rows 8-15)          way 1  k 0-3 : one m16n8k4
 //   way 2  k 0-7 : two chained m16n8k4                       way 3  k 0-7 : one m16n8k8
 //   way 4  k 0-15: four chained m16n8k4                      way 5  k 0-15: one m16n8k16
+//   way 6  k 0-3 : d = fma(a3, b3, fma(a2, b2, fma(a1, b1, fma(a0, b0, c))))      way 7  k 0-15: the same chain, 16 long
+#define NWAYS 8
 __global__ void k_bits(const double *A, const double *B, const double *C, double *out) {
   const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
   const double *Aw = A + (size_t)w * 256, *Bw = B + (size_t)w * 128, *Cw = C + (size_t)w * 128;
-  double *ow = out + (size_t)w * 6 * 128;
+  double *ow = out + (size_t)w * NWAYS * 128;
   auto ldc = [&](double *c) { c[0] = Cw[g * 8 + 2 * q]; c[1] = Cw[g * 8 + 2 * q + 1]; c[2] = Cw[(g + 8) * 8 + 2 * q]; c[3] = Cw[(g + 8) * 8 + 2 * q + 1]; };
   auto stc = [&](int way, const double *c) {
     double *o = ow + way * 128;
@@ -129,6 +133,16 @@ __global__ void k_bits(const double *A, const double *B, const double *C, double
     stc(4, c);
   }
   { ldc(c); for (int i = 0; i < 8; i++) a[i] = lda(i, 0); for (int j = 0; j < 4; j++) b[j] = ldb(j, 0); mma16816(c, a, b); stc(5, c); }
+  for (int way = 6; way < 8; way++) { // this lane's four outputs C[g + 8h][2q + e], h = u >> 1, e = u & 1
+    const int kmax = way == 6 ? 4 : 16;
+    ldc(c);
+    for (int u = 0; u < 4; u++) {
+      const int r = g + 8 * (u >> 1), n = 2 * q + (u & 1);
+      for (int k = 0; k < kmax; k++)
+        c[u] = __fma_rn(Aw[r * 16 + k], Bw[k * 8 + n], c[u]);
+    }
+    stc(way, c);
+  }
 }
 
 #define CK(x) do { cudaError_t e = (x); if (e != cudaSuccess) { printf("CUDA error %s at %d\n", cudaGetErrorString(e), __LINE__); return 1; } } while (0)
@@ -190,14 +204,14 @@ int main() {
 
   // ---- bit identity: 3 input families x NW warps each
   const int NW = 8192;
-  std::vector<double> hA((size_t)NW * 256), hB((size_t)NW * 128), hC((size_t)NW * 128), hD((size_t)NW * 6 * 128);
+  std::vector<double> hA((size_t)NW * 256), hB((size_t)NW * 128), hC((size_t)NW * 128), hD((size_t)NW * NWAYS * 128);
   double *dA, *dB, *dC, *dD;
   CK(cudaMalloc(&dA, hA.size() * 8)); CK(cudaMalloc(&dB, hB.size() * 8)); CK(cudaMalloc(&dC, hC.size() * 8)); CK(cudaMalloc(&dD, hD.size() * 8));
   std::mt19937_64 rng(20261018);
   std::uniform_real_distribution<double> U(-1.0, 1.0);
   std::uniform_int_distribution<int> E(-30, 30);
   const char *fam[3] = {"uniform [-1,1]", "wide exponents 2^+-30", "cancellation"};
-  int total_bad = 0;
+  long total_bad = 0, total_dfma_bad = 0;
   for (int f = 0; f < 3; f++) {
     for (int w = 0; w < NW; w++) {
       double *A = &hA[(size_t)w * 256], *B = &hB[(size_t)w * 128], *C = &hC[(size_t)w * 128];
@@ -224,16 +238,25 @@ int main() {
     k_bits<<<NW / 4, 128>>>(dA, dB, dC, dD);
     CK(cudaGetLastError());
     CK(cudaMemcpy(hD.data(), dD, hD.size() * 8, cudaMemcpyDeviceToHost));
-    long bad[3] = {0, 0, 0};
+    // pairs of ways that must agree; the last three compare the tensor core with the scalar FMA chain, element by element
+    const int pairs[6][2] = {{0, 1}, {2, 3}, {4, 5}, {0, 6}, {1, 6}, {4, 7}};
+    long bad[6] = {0, 0, 0, 0, 0, 0};
     for (int w = 0; w < NW; w++) {
-      const double *o = &hD[(size_t)w * 6 * 128];
+      const double *o = &hD[(size_t)w * NWAYS * 128];
       for (int pr = 0; pr < 3; pr++)
-        if (memcmp(o + 2 * pr * 128, o + (2 * pr + 1) * 128, 128 * 8) != 0) bad[pr]++;
+        if (memcmp(o + pairs[pr][0] * 128, o + pairs[pr][1] * 128, 128 * 8) != 0) bad[pr]++;
+      for (int pr = 3; pr < 6; pr++)
+        for (int e = 0; e < 128; e++)
+          if (memcmp(o + pairs[pr][0] * 128 + e, o + pairs[pr][1] * 128 + e, 8) != 0) bad[pr]++;
     }
     printf("bits [%s], %d warps: m16n8k4 != 2x m8n8k4: %ld   m16n8k8 != 2x m16n8k4: %ld   m16n8k16 != 4x m16n8k4: %ld\n", fam[f], NW,
            bad[0], bad[1], bad[2]);
+    printf("bits [%s], %d outputs: m8n8k4 != 4 chained DFMA: %ld   m16n8k4 != 4 chained DFMA: %ld   4x m16n8k4 != 16 chained DFMA: %ld\n",
+           fam[f], NW * 128, bad[3], bad[4], bad[5]);
     total_bad += bad[0] + bad[1] + bad[2];
+    total_dfma_bad += bad[3] + bad[4] + bad[5];
   }
   printf("bit identity: %s\n", total_bad ? "DIFFERS" : "all identical");
+  printf("DMMA against chained DFMA: %s\n", total_dfma_bad ? "DIFFERS" : "all identical");
   return 0;
 }
